@@ -13,7 +13,7 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_SRC = "/root/reference"
+REF_SRC = os.environ.get("SLB200_REFERENCE_DIR", "")   # checkout of the reference repository
 DST = os.path.join(HERE, "_ref")
 
 
@@ -25,8 +25,8 @@ def _sha(path):
 def install(force=False):
     if os.path.exists(os.path.join(DST, "MANIFEST.json")) and not force:
         return DST
-    if not os.path.isdir(REF_SRC):
-        raise RuntimeError("reference source not mounted")
+    if not REF_SRC or not os.path.isdir(REF_SRC):
+        raise RuntimeError("set SLB200_REFERENCE_DIR to a checkout of the reference repository")
     tmp = "/tmp/_slb200_refcopy"
     shutil.rmtree(tmp, ignore_errors=True)
     shutil.copytree(REF_SRC, tmp, ignore=shutil.ignore_patterns(".git", "other", "pics"))

@@ -31,7 +31,7 @@ def _prepare_imports():
     ref = install()
     man = json.load(open(os.path.join(ref, "MANIFEST.json")))
     if not all(v["matches_reference"] for v in man["files"].values()):
-        raise RuntimeError("baseline/_ref differs from /root/reference")
+        raise RuntimeError("baseline/_ref differs from the reference tree")
     for p in (ref, os.path.join(HERE, "shims")):
         if p in sys.path:
             sys.path.remove(p)

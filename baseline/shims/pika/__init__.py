@@ -11,7 +11,7 @@ Message-completion hook: ``on_get`` callbacks let the benchmark harness observe 
 
 NCCL mode (``use_nccl``; ``bench.py --impl reference-nccl``) — the "reference's own NCCL build" that BASELINE.json names as
 the competitor: the tensors of the two HOT queues (``intermediate_queue_*`` activations, ``gradient_queue_*`` gradients,
-/root/reference/src/train/VGG16.py:20-53) travel GPU -> GPU with ``torch.distributed`` NCCL ``isend`` / ``recv``; only a small
+reference src/train/VGG16.py:20-53) travel GPU -> GPU with ``torch.distributed`` NCCL ``isend`` / ``recv``; only a small
 header (data_id, label, trace, shape) goes through the broker, and the control verbs stay on the broker as before.  The
 reference trainers are untouched: they still hand the shim a pickled dict with a CPU NumPy array and get one back, so the
 D2H / H2D copies at the trainer boundary remain (they are part of the reference's code), but the wire itself is NCCL p2p

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline benchmark: VGG16/CIFAR10 split-learning throughput (images/s) on N B200s.
+"""Headline benchmark: VGG16/CIFAR10 split-learning throughput (images/s) on N H100s.
 
     python bench.py --gpus N --steps K --warmup W            # this framework
     python bench.py --impl reference --gpus N ...            # unmodified reference (baseline/_ref)
@@ -8,15 +8,20 @@ Config (BASELINE.json): VGG16_CIFAR10 cut at layer 7, microbatch 32, control-cou
 SGD(lr 5e-4, momentum 0.5); N = 1 → both stages on one GPU, N = 2 → one GPU per stage,
 N = 4/8 → N/2 replicas per stage (independent 1:1 chains, FedAvg at round end, outside the
 timed steps as in the reference).  Weak scaling: every first-stage replica processes its own
-32-image microbatches.  Synthetic CIFAR-10-shaped data, random-init weights, bf16 tensor-core
-compute with fp32 master weights / accumulation.
+32-image microbatches.  Synthetic CIFAR-10-shaped data (seeded: identical inputs from run to run),
+random-init weights, tf32 tensor-core convolutions with fp32 accumulation (``--precision bf16``:
+bf16 activations with fp32 master weights).
 
 Timing: W warm-up steps, then exactly K steps between barrier + cuda synchronize, CUDA events
 on the launching stream, max over ranks.  ``value`` = device-resident inputs (kernel pipeline
 only); ``e2e`` = same K steps through ``LocalPipeline.run`` / the stage runner with a pinned
 host→device copy of every microbatch and a device→host read of every step's loss.
 The per-step working set (fp32 master + momentum + gradient + bf16 shadow ≈ 470 MB/stage-2
-replica) exceeds the 126 MB L2, so no explicit L2 flush is needed between iterations.
+replica) exceeds the 50 MB L2, so no explicit L2 flush is needed between iterations.
+
+``--dump-outputs DIR`` (N = 1): after the timed steps, write what the last timed step computed as
+DIR/<name>.npy (float32): the loss, the activation that crossed each cut and the gradient that came
+back (NCHW), and a fixed seeded sample of every stage's updated fp32 parameters.
 """
 from __future__ import annotations
 
@@ -43,7 +48,7 @@ def parse():
     ap.add_argument("--cut", type=int, default=7)
     ap.add_argument("--cuts", default=None, help="N=1 only: comma list for an N-stage pipeline on one GPU, e.g. 5,10")
     ap.add_argument("--precision", default="tf32", choices=["tf32", "bf16"],
-                    help="tf32 (default) = the reference's precision: fp32 tensors, tcgen05 kind::tf32 convolutions with fp32 "
+                    help="tf32 (default) = the reference's precision: fp32 tensors, wgmma tf32 convolutions with fp32 "
                          "accumulation, fp32 Linear/BN/SGD; bf16 = opt-in fast mode")
     ap.add_argument("--placement", default="ring", choices=["ring", "split"],
                     help="N > 1: ring = N chains, GPU r hosts stage 1 of chain r and stage 2 of chain r-1 (default; per-GPU work "
@@ -58,11 +63,16 @@ def parse():
     ap.add_argument("--timeout", type=float, default=1500.0)
     ap.add_argument("--breakdown", action="store_true", help="also report device time per stage program (F / L / B)")
     ap.add_argument("--no-overlap", action="store_true", help="N=1: run both stages on one stream")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="N=1: write the outputs of the last timed step to DIR/<name>.npy (compare two builds output for output)")
+    args = ap.parse_args()
+    if args.dump_outputs and (args.gpus > 1 or args.scenario or args.impl != "ours"):
+        ap.error("--dump-outputs is supported for --gpus 1 --impl ours without --scenario")
+    return args
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -108,7 +118,7 @@ class ClockSampler:
 
 
 DTYPE_LABEL = {
-    "tf32": "fp32 tensors; conv = tcgen05 kind::tf32 with fp32 accumulate (the reference's cuDNN-TF32 default), "
+    "tf32": "fp32 tensors; conv = wgmma tf32 with fp32 accumulate (the reference's cuDNN-TF32 default), "
             "Linear/BN/CE/SGD = fp32",
     "bf16": "bf16 activations + bf16 weight shadow, fp32 master/accumulate (opt-in fast mode)",
 }
@@ -123,6 +133,27 @@ def synthetic_batches(n: int, batch: int, seed: int):
         y = torch.randint(0, 10, (batch,), generator=g).pin_memory()
         out.append((x, y))
     return out
+
+
+PARAM_SAMPLE = 1 << 21          # parameters per stage in a --dump-outputs sample (8 MB of float32)
+
+
+def dump_outputs(out_dir: str, pipe, exs, last_it: int) -> None:
+    """What the last timed step (microbatch ``last_it``) handed back to the caller of the pipeline, as float32 .npy files."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    path = lambda name: os.path.join(out_dir, name + ".npy")
+    slot = last_it % pipe.depth
+    np.save(path("loss"), pipe.loss()[:1].float().cpu().numpy())
+    for i, st in enumerate(pipe.stages[:-1]):
+        np.save(path(f"cut{i}_activation"), st.fwd_out.payload[slot].float().permute(0, 3, 1, 2).cpu().numpy())
+        np.save(path(f"cut{i}_gradient"), st.grad_in.payload[slot].float().permute(0, 3, 1, 2).cpu().numpy())
+    rng = np.random.default_rng(0)
+    for i, ex in enumerate(exs):
+        n = ex.P.numel()
+        idx = np.sort(rng.choice(n, min(n, PARAM_SAMPLE), replace=False))
+        np.save(path(f"stage{i}_params_sample"), ex.P[torch.from_numpy(idx).to(ex.P.device)].float().cpu().numpy())
 
 
 def run_ours(args) -> dict:
@@ -206,6 +237,8 @@ def run_ours(args) -> dict:
     ms_e2e = f0.elapsed_time(f1)
     clocks = sampler.stop(t0, t1)
     pipe.synchronize()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, pipe, exs, pipe.it_f - 1)
     breakdown = None
     if args.breakdown:
         evs = []
@@ -242,7 +275,7 @@ def run_ours(args) -> dict:
                    "parallelism": f"pp{len(cuts) + 1} (all stages on one GPU, one stream per stage)",
                    "optimizer": "SGD lr=5e-4 momentum=0.5, step per microbatch", "recompute": True,
                    "cuda_graphs": not args.no_graphs,
-                   "l2": "per-step working set ~470 MB (fp32 master+momentum+grad+bf16 shadow) > 126 MB L2; no flush needed"},
+                   "l2": "per-step working set ~470 MB (fp32 master+momentum+grad+bf16 shadow) > 50 MB L2; no flush needed"},
         "e2e": {"value": K * B / (ms_e2e / 1e3), "unit": "images/s", "ms_per_step": ms_e2e / K,
                 "h2d_bytes_per_step": B * 3 * 32 * 32 * 4 + B * 8, "d2h_bytes_per_step": 16},
         "gpu_launches": per_step * K, "launches_per_step": per_step, "clocks": clocks, "final_loss": loss, "impl": "ours",

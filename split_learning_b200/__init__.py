@@ -1,4 +1,4 @@
-"""split_learning_b200 — a Blackwell-native split-learning engine (see DESIGN.md)."""
+"""split_learning_b200 — a Hopper-native (H100) split-learning engine (see DESIGN.md)."""
 __version__ = "0.1.0"
 
 import os as _os

@@ -23,7 +23,7 @@ DEFAULT_LEARNING = {
 }
 
 DEFAULT_B200 = {
-    # "auto" → sm_100a kernels on CUDA, reference-math torch executor on CPU
+    # "auto" → sm_90a kernels on CUDA, reference-math torch executor on CPU
     "executor": "auto",
     # faithful = recompute forward at backward time on non-last stages (reference semantics,
     # src/train/VGG16.py:89-92); "stash" keeps activations instead

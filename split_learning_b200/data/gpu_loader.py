@@ -2,7 +2,7 @@
 
 The reference builds every microbatch on the host: PIL crop / flip / ToTensor / Normalize per sample in a
 ``DataLoader`` (src/dataset/dataloader.py:61-84), then ``.to(device)``.  CIFAR-10 is 150 MB of uint8 — it fits in a
-corner of a B200's HBM — so here the selected training subset lives on the GPU once and each microbatch is ONE kernel
+corner of an H100's 80 GB of HBM — so here the selected training subset lives on the GPU once and each microbatch is ONE kernel
 (``image_batch_kernel``): gather by shuffled index, RandomCrop(32, padding 4), RandomHorizontalFlip, /255, Normalize,
 written as the fp32 NCHW stage input.  No host work and no H2D copy per step; the iterator yields device tensors, which
 every executor and the device data plane accept as they are.

@@ -64,7 +64,7 @@ class SyntheticDataset(Dataset):
 class BatchedTensorLoader:
     """Loader for a dataset that is already a pair of in-memory tensors: one ``index_select`` per microbatch straight into a
     page-locked staging slot instead of ``batch_size`` ``__getitem__`` calls + ``default_collate`` (≈0.3 ms per CIFAR
-    microbatch with ``torch.utils.data.DataLoader``, which is the whole device time of a first-stage step on a B200).
+    microbatch with ``torch.utils.data.DataLoader``, comparable to the whole device time of a first-stage step).
     Same iteration contract as ``DataLoader(ds, batch_size, shuffle, drop_last=False)``: a fresh permutation per epoch, the
     short batch last.  ``pin=True`` yields pinned slots, one per microbatch of an epoch (epochs of up to
     ``MAX_PINNED_BATCHES`` microbatches; longer ones yield pageable tensors) — a slot is rewritten one epoch later, after the

@@ -6,7 +6,7 @@ weight), fp32 accumulation, NaN → 0 before weighting, integer/bool tensors rou
 their dtype (this is how ``num_batches_tracked`` survives).  ``fedasync_merge`` is the
 2LS running merge (other/2LS/src/Server.py:224-233).
 
-On CUDA the per-key loop is replaced by one flat pass through the fused sm_100a kernel
+On CUDA the per-key loop is replaced by one flat pass through the fused sm_90a kernel
 (``ops.fedavg_flat``); across GPUs ``parallel.fedavg_allreduce`` performs the same math
 in place over NVLink peer memory.
 """

@@ -8,7 +8,7 @@ state-dict keys are globally unique and a full-model checkpoint is just the
 union of the stage dicts (reference behaviour: src/model/VGG16_CIFAR10.py:4-117,
 src/Server.py:410-434).
 
-The same table is what the B200 stage executor compiles into a fused kernel
+The same table is what the native stage executor compiles into a fused kernel
 plan (``split_learning_b200/train/b200_executor.py``), so models are *data*
 here, not code.
 """

@@ -1,4 +1,4 @@
-"""Build the sm_100a kernel library in-tree: ``ops/_slb200.so`` (plain C ABI, loaded by
+"""Build the sm_90a kernel library in-tree: ``ops/_slb200.so`` (plain C ABI, loaded by
 ctypes — no torch headers, seconds to compile, and it travels to the GPU box with the tree).
 
     python -m split_learning_b200.ops.build [--force]
@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["umma_gemm.cu", "fused_cut.cu", "elementwise.cu", "transformer.cu", "allreduce.cu", "ticket.cu", "peer.cu"]
 LIB = os.path.join(HERE, "_slb200.so")
 STAMP = LIB + ".sha"
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--shared", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-lcudart"] + os.environ.get("SLB200_NVCC_EXTRA", "").split()
 
 

@@ -11,7 +11,7 @@
 // only.  Weights, NaN votes and both barriers live in device memory (st.release.sys / ld.acquire.sys flags in each
 // participant's exported sync block): no host message, pickle or NCCL call is involved in a round.
 // Integer state (num_batches_tracked mirrors) is rounded to the nearest integer in the same pass.
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace slb {
 

@@ -3,9 +3,95 @@
 // (Cin <= 4), Linear finalisation (bias/ReLU/dropout), fused CE forward+backward, fused
 // flat optimisers (SGD-momentum, AdamW), the FedAvg weighted n-ary reduction over (peer)
 // pointers, and the mailbox flag primitives.  All vectorised to 16-byte accesses.
-#include "sm100.cuh"
+#include "sm90.cuh"
+
+#include <map>
+#include <mutex>
+#include <utility>
+#include <vector>
 
 namespace slb {
+
+// ============================================================================ per-stream reduction scratch (sm90.cuh Det)
+// A stream gets its scratch when this library creates it (slb_stream_create) or first uses it outside a CUDA-graph capture:
+// its own allocation, counters zeroed by a memset ordered before its first reduction.  Inside a capture (torch records
+// graphs on a side stream) nothing may be allocated or memset, so a stream first seen there takes a pre-zeroed slot from
+// the device's reserve, filled at the first use outside a capture.  Slots go back (or are freed) when the stream is destroyed.
+constexpr long long DET_PART_FLOATS = 1ll << 20;  // 4 MB of partial rows per stream
+constexpr size_t DET_CTR_BYTES = static_cast<size_t>(DET_COUNTERS) * sizeof(uint32_t);
+constexpr int DET_RESERVE = 32;
+struct DetSlot {
+  Det d;
+  bool owned;           // own allocation (freed with the stream) or a reserve slot (returned)
+};
+static std::mutex g_det_mu;
+static std::map<std::pair<int, cudaStream_t>, DetSlot> g_det_slots;
+static std::map<int, std::vector<Det>> g_det_reserve;
+static std::map<int, bool> g_det_reserve_filled;
+
+// caller holds g_det_mu; st is not capturing
+static bool det_fill_reserve(int dev, cudaStream_t st) {
+  if (g_det_reserve_filled[dev]) return true;
+  float* part = nullptr;
+  uint32_t* ctr = nullptr;
+  if (cudaMalloc(reinterpret_cast<void**>(&part), DET_RESERVE * DET_PART_FLOATS * sizeof(float)) != cudaSuccess) return false;
+  if (cudaMalloc(reinterpret_cast<void**>(&ctr), DET_RESERVE * DET_CTR_BYTES) != cudaSuccess ||
+      cudaMemsetAsync(ctr, 0, DET_RESERVE * DET_CTR_BYTES, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
+    cudaFree(part);
+    return false;
+  }
+  for (int i = DET_RESERVE - 1; i >= 0; --i)
+    g_det_reserve[dev].push_back({part + i * DET_PART_FLOATS, ctr + static_cast<long long>(i) * DET_COUNTERS, DET_PART_FLOATS});
+  g_det_reserve_filled[dev] = true;
+  return true;
+}
+
+Det slb_det(cudaStream_t st) {
+  const Det none = {nullptr, nullptr, 0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) return none;
+  std::lock_guard<std::mutex> lock(g_det_mu);
+  auto it = g_det_slots.find({dev, st});
+  if (it != g_det_slots.end()) return it->second.d;
+  if (cs != cudaStreamCaptureStatusNone) {
+    std::vector<Det>& res = g_det_reserve[dev];
+    if (res.empty()) return none;
+    const Det d = res.back();
+    res.pop_back();
+    g_det_slots[{dev, st}] = {d, false};
+    return d;
+  }
+  if (!det_fill_reserve(dev, st)) return none;
+  float* part = nullptr;
+  uint32_t* ctr = nullptr;
+  if (cudaMalloc(reinterpret_cast<void**>(&part), DET_PART_FLOATS * sizeof(float)) != cudaSuccess) return none;
+  if (cudaMalloc(reinterpret_cast<void**>(&ctr), DET_CTR_BYTES) != cudaSuccess ||
+      cudaMemsetAsync(ctr, 0, DET_CTR_BYTES, st) != cudaSuccess) {
+    cudaFree(part);
+    return none;
+  }
+  const Det d = {part, ctr, DET_PART_FLOATS};
+  g_det_slots[{dev, st}] = {d, true};
+  return d;
+}
+
+void slb_det_release(cudaStream_t st) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lock(g_det_mu);
+  auto it = g_det_slots.find({dev, st});
+  if (it == g_det_slots.end()) return;
+  cudaStreamSynchronize(st);
+  if (it->second.owned) {
+    cudaFree(it->second.d.part);
+    cudaFree(it->second.d.ctr);
+  } else {
+    g_det_reserve[dev].push_back(it->second.d);      // counters are zero at rest
+  }
+  g_det_slots.erase(it);
+}
 
 struct alignas(16) bf16x8 { __nv_bfloat162 v[4]; };
 
@@ -236,6 +322,7 @@ struct BnBwdParams {
   int P, C, H, W;
   int relu, pool;
   int identity;
+  Det det;                     // reproducible dgamma / dbeta reduction
 };
 
 // dz for the 1 (no pool) or 4 (pool) input pixels of output position `op`, 8 channels.
@@ -314,16 +401,18 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const BnBwdParams<T>
   extern __shared__ float s_red[];            // [2][C]
   for (int i = threadIdx.y * blockDim.x + threadIdx.x; i < 2 * p.C; i += blockDim.x * blockDim.y) s_red[i] = 0.f;
   __syncthreads();
+  for (int r = 0; r < static_cast<int>(blockDim.y); ++r) {     // rows in order: a reproducible sum
+    if (threadIdx.y == r) {
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    atomicAdd(&s_red[g * 8 + j], ag[j]);
-    atomicAdd(&s_red[p.C + g * 8 + j], ab[j]);
+      for (int j = 0; j < 8; ++j) {
+        s_red[g * 8 + j] += ag[j];
+        s_red[p.C + g * 8 + j] += ab[j];
+      }
+    }
+    __syncthreads();
   }
-  __syncthreads();
-  for (int i = threadIdx.y * blockDim.x + threadIdx.x; i < p.C; i += blockDim.x * blockDim.y) {
-    atomicAdd(p.dgamma + i, s_red[i]);
-    atomicAdd(p.dbeta + i, s_red[p.C + i]);
-  }
+  det_commit<-1>(p.det, 0, blockIdx.x, gridDim.x, s_red, 2 * p.C, p.dgamma, p.C, p.dbeta,
+                 threadIdx.y * blockDim.x + threadIdx.x, blockDim.x * blockDim.y);
 }
 
 // pass 2: dy = gamma*invstd*(dz - dbeta/P - xhat*dgamma/P)
@@ -483,16 +572,18 @@ __global__ void __launch_bounds__(256, 2) bn_bwd_fused_kernel(const BnBwdParams<
   extern __shared__ float s_red[];            // [2][C]
   for (int i = threadIdx.y * blockDim.x + threadIdx.x; i < 2 * p.C; i += blockDim.x * blockDim.y) s_red[i] = 0.f;
   __syncthreads();
+  for (int r = 0; r < static_cast<int>(blockDim.y); ++r) {     // rows in order: a reproducible sum
+    if (threadIdx.y == r) {
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    atomicAdd(&s_red[g * 8 + j], ag[j]);
-    atomicAdd(&s_red[p.C + g * 8 + j], ab[j]);
+      for (int j = 0; j < 8; ++j) {
+        s_red[g * 8 + j] += ag[j];
+        s_red[p.C + g * 8 + j] += ab[j];
+      }
+    }
+    __syncthreads();
   }
-  __syncthreads();
-  for (int i = threadIdx.y * blockDim.x + threadIdx.x; i < p.C; i += blockDim.x * blockDim.y) {
-    atomicAdd(p.dgamma + i, s_red[i]);
-    atomicAdd(p.dbeta + i, s_red[p.C + i]);
-  }
+  det_commit<-1>(p.det, 0, blockIdx.x, gridDim.x, s_red, 2 * p.C, p.dgamma, p.C, p.dbeta,
+                 threadIdx.y * blockDim.x + threadIdx.x, blockDim.x * blockDim.y);
   // ---- grid barrier ----
   __syncthreads();
   if (leader) {
@@ -542,7 +633,7 @@ __global__ void __launch_bounds__(256, 2) bn_bwd_fused_kernel(const BnBwdParams<
 
 // Column sums / sums of squares of an activation-typed [P][C] matrix (BN statistics fallback, bias gradients).
 template <typename T>
-__global__ void __launch_bounds__(256) col_stats_kernel(const T* y, float* sum, float* sumsq, long long P, int C) {
+__global__ void __launch_bounds__(256) col_stats_kernel(const T* y, float* sum, float* sumsq, long long P, int C, const Det det) {
   pdl_trigger();
   pdl_wait();
   const int g = threadIdx.x;
@@ -558,23 +649,25 @@ __global__ void __launch_bounds__(256) col_stats_kernel(const T* y, float* sum, 
   extern __shared__ float s_red[];
   for (int i = threadIdx.y * blockDim.x + threadIdx.x; i < 2 * C; i += blockDim.x * blockDim.y) s_red[i] = 0.f;
   __syncthreads();
+  for (int r = 0; r < static_cast<int>(blockDim.y); ++r) {     // rows in order: a reproducible sum
+    if (threadIdx.y == r) {
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    atomicAdd(&s_red[g * 8 + j], a[j]);
-    atomicAdd(&s_red[C + g * 8 + j], b[j]);
+      for (int j = 0; j < 8; ++j) {
+        s_red[g * 8 + j] += a[j];
+        s_red[C + g * 8 + j] += b[j];
+      }
+    }
+    __syncthreads();
   }
-  __syncthreads();
-  for (int i = threadIdx.y * blockDim.x + threadIdx.x; i < C; i += blockDim.x * blockDim.y) {
-    atomicAdd(sum + i, s_red[i]);
-    if (sumsq) atomicAdd(sumsq + i, s_red[C + i]);
-  }
+  det_commit<-1>(det, 0, blockIdx.x, gridDim.x, s_red, sumsq ? 2 * C : C, sum, C, sumsq, threadIdx.y * blockDim.x + threadIdx.x,
+                 blockDim.x * blockDim.y);
 }
 
-// Split-K epilogue of the tcgen05 conv: y = bf16(acc + bias) and the BN statistics of the rounded values
+// Split-K epilogue of the wgmma conv: y = bf16(acc + bias) and the BN statistics of the rounded values
 // (acc: fp32 [P][C] partial-sum buffer filled with red.add by the K-slices).  bias/y/sum may be null.
 template <typename T>
 __global__ void __launch_bounds__(256) conv_finalize_kernel(const float* acc, const float* bias, T* y, float* sum,
-                                                           float* sumsq, long long P, int C) {
+                                                           float* sumsq, long long P, int C, const Det det) {
   pdl_trigger();
   pdl_wait();
   const int g = threadIdx.x;
@@ -598,16 +691,18 @@ __global__ void __launch_bounds__(256) conv_finalize_kernel(const float* acc, co
   extern __shared__ float s_red[];
   for (int i = threadIdx.y * blockDim.x + threadIdx.x; i < 2 * C; i += blockDim.x * blockDim.y) s_red[i] = 0.f;
   __syncthreads();
+  for (int r = 0; r < static_cast<int>(blockDim.y); ++r) {     // rows in order: a reproducible sum
+    if (threadIdx.y == r) {
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    atomicAdd(&s_red[g * 8 + j], a[j]);
-    atomicAdd(&s_red[C + g * 8 + j], b[j]);
+      for (int j = 0; j < 8; ++j) {
+        s_red[g * 8 + j] += a[j];
+        s_red[C + g * 8 + j] += b[j];
+      }
+    }
+    __syncthreads();
   }
-  __syncthreads();
-  for (int i = threadIdx.y * blockDim.x + threadIdx.x; i < C; i += blockDim.x * blockDim.y) {
-    atomicAdd(sum + i, s_red[i]);
-    atomicAdd(sumsq + i, s_red[C + i]);
-  }
+  det_commit<-1>(det, 0, blockIdx.x, gridDim.x, s_red, 2 * C, sum, C, sumsq, threadIdx.y * blockDim.x + threadIdx.x,
+                 blockDim.x * blockDim.y);
 }
 
 // ============================================================================ first-layer direct conv (Cin <= 4)
@@ -632,7 +727,7 @@ __device__ __forceinline__ float warp_col_reduce32e(float (&v)[32]) {
 template <int CIN, int COUT, typename T>
 __global__ void __launch_bounds__(128) conv3x3_small_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                                const float* __restrict__ bias, T* y,
-                                                               float* sum, float* sumsq, int B, int H, int W) {
+                                                               float* sum, float* sumsq, int B, int H, int W, const Det det) {
   pdl_trigger();
   pdl_wait();
   constexpr int KK = 9 * CIN;
@@ -683,17 +778,16 @@ __global__ void __launch_bounds__(128) conv3x3_small_fwd_kernel(const float* __r
       }
       const float c1 = warp_col_reduce32e(s1);
       const float c2 = warp_col_reduce32e(s2);
-      atomicAdd(&s_st[c0 + (threadIdx.x & 31)], c1);
-      atomicAdd(&s_st[COUT + c0 + (threadIdx.x & 31)], c2);
+      for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) {   // warps in order: a reproducible sum
+        if ((threadIdx.x >> 5) == w) {
+          s_st[c0 + (threadIdx.x & 31)] += c1;
+          s_st[COUT + c0 + (threadIdx.x & 31)] += c2;
+        }
+        __syncthreads();
+      }
     }
   }
-  if (sum) {
-    __syncthreads();
-    for (int i = threadIdx.x; i < COUT; i += blockDim.x) {
-      atomicAdd(sum + i, s_st[i]);
-      atomicAdd(sumsq + i, s_st[COUT + i]);
-    }
-  }
+  if (sum) det_commit<-1>(det, 0, blockIdx.x, gridDim.x, s_st, 2 * COUT, sum, COUT, sumsq, threadIdx.x, blockDim.x);
 }
 
 // dw[Cout][9*CIN] += sum_pix dy[pix][Cout] * patch[pix][9*CIN]  (first conv of the network: CIN = 3 or 1, Cout <= 64).
@@ -704,7 +798,7 @@ __global__ void __launch_bounds__(128) conv3x3_small_fwd_kernel(const float* __r
 // the pixel slices are combined with shared-memory atomics, then one global red per output and block.
 template <int CIN, typename T>
 __global__ void __launch_bounds__(256) conv3x3_small_wgrad_kernel(const float* __restrict__ x, const T* __restrict__ dy,
-                                                                 float* dw, int B, int H, int W, int Cout) {
+                                                                 float* dw, int B, int H, int W, int Cout, const Det det) {
   pdl_trigger();
   pdl_wait();
   constexpr int KK = 9 * CIN;
@@ -763,17 +857,18 @@ __global__ void __launch_bounds__(256) conv3x3_small_wgrad_kernel(const float* _
       }
     }
   }
-  if (active) {
+  for (int sl = 0; sl < slices; ++sl) {                           // pixel slices in order: a reproducible sum
+    if (active && slice == sl) {
 #pragma unroll
-    for (int a = 0; a < 4; ++a)
+      for (int a = 0; a < 4; ++a)
 #pragma unroll
-      for (int j = 0; j < KG; ++j) atomicAdd(s_out + (cg * 4 + a) * KP + kg * KG + j, acc[a][j]);
+        for (int j = 0; j < KG; ++j) s_out[(cg * 4 + a) * KP + kg * KG + j] += acc[a][j];
+    }
+    __syncthreads();
   }
+  for (int i = threadIdx.x; i < Cout * KK; i += blockDim.x) s_patch[i] = s_out[(i / KK) * KP + i % KK];   // drop the padding
   __syncthreads();
-  for (int i = threadIdx.x; i < Cout * KP; i += blockDim.x) {
-    const int co = i / KP, k = i - co * KP;
-    if (k < KK) atomicAdd(dw + co * KK + k, s_out[i]);
-  }
+  det_commit<-1>(det, 0, blockIdx.x, gridDim.x, s_patch, Cout * KK, dw, Cout * KK, nullptr, threadIdx.x, blockDim.x);
 }
 
 // ============================================================================ Linear finalisation
@@ -867,9 +962,8 @@ __global__ void dropout_bwd_kernel(const float* dacc, const uint8_t* mask, T* dx
 // (16 FLOP per weight byte): the kernels below read every weight exactly once with 16-byte coalesced loads and keep the
 // whole batch tile in registers / shared memory.
 
-// Packed fp32 FMA (FFMA2 on sm_100: two IEEE round-to-nearest fp32 FMAs per instruction, same results as two fmaf) — the
-// 3-register FFMA issues every second cycle per scheduler, so the scalar versions of these kernels sat at ~2x their
-// 37 TFLOP/s bound; pairing two batch rows per instruction halves the issue slots.
+// Two batch rows per accumulator pair: f32x2 packs (row 2bp, row 2bp + 1); ffma2 is two IEEE round-to-nearest fp32 FMAs
+// (sm_90 has no packed fp32 FMA instruction, so it is two FFMAs).
 // Ampere-style asynchronous copies (LDGSTS): the weight stream of the fp32 Linear kernels is staged through a ring of
 // shared-memory stages so that several steps of HBM traffic are in flight per SM without holding registers (ncu on the
 // register-prefetch version: 22 % of the stall samples on the first use of the prefetched weights, DRAM at 13 % of peak).
@@ -888,16 +982,19 @@ __device__ __forceinline__ f32x2 pack2(float lo, float hi) {
 }
 __device__ __forceinline__ void unpack2(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
 __device__ __forceinline__ f32x2 ffma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  unpack2(c, c0, c1);
+  return pack2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 
 // acc[b][n] (+)= sum_{k in slice} x[b][k] * w[n][k]            grid (ceil(N/32), ceil(K/kc), ceil(B/32)), 256 threads
 // warp = (feature group of 8) x (batch half of 16); lanes stride K in float4 steps; partial sums are reduced across the
 // warp with the register butterfly and added to `acc` (zeroed by the caller) with one atomic per (b, n) per slice.
 __global__ void __launch_bounds__(256) linear_fwd_f32_kernel(const float* __restrict__ x, const float* __restrict__ w,
-                                                            float* acc, int B, int N, int K, int ldx, int ldw, int lda, int kc) {
+                                                            float* acc, int B, int N, int K, int ldx, int ldw, int lda, int kc,
+                                                            const Det det) {
   pdl_trigger();
   pdl_wait();
   constexpr int ST = 4;                                          // weight stages in flight (16 KB each)
@@ -986,11 +1083,24 @@ __global__ void __launch_bounds__(256) linear_fwd_f32_kernel(const float* __rest
   for (int f = 0; f < 8; ++f)
 #pragma unroll
     for (int bp = 0; bp < 8; ++bp) unpack2(ac2[f][bp], a[f >> 1][(f & 1) * 16 + 2 * bp], a[f >> 1][(f & 1) * 16 + 2 * bp + 1]);
+  float v[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) v[q] = warp_col_reduce32e(a[q]);  // lane j: sum over lanes of a[q][j]
+  // K slices add in slice order (blockIdx.y) behind a turn counter: the same sum every run
+  uint32_t* turn = det.ctr + DET_TURN_BASE + blockIdx.z * gridDim.x + blockIdx.x;
+  if (gridDim.y > 1) {
+    if (threadIdx.x == 0) turn_wait(turn, blockIdx.y);
+    __syncthreads();
+  }
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    const float v = warp_col_reduce32e(a[q]);                    // lane j: sum over lanes of a[q][j]
     const int f = 2 * q + (lane >> 4), b = b0 + bh * 16 + (lane & 15);
-    if (n0 + f < N && b < B) atomicAdd(acc + (long long)b * lda + n0 + f, v);
+    if (n0 + f < N && b < B) atomicAdd(acc + (long long)b * lda + n0 + f, v[q]);
+  }
+  if (gridDim.y > 1) {
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) turn_pass(turn, blockIdx.y, gridDim.y);
   }
 }
 
@@ -998,7 +1108,8 @@ __global__ void __launch_bounds__(256) linear_fwd_f32_kernel(const float* __rest
 // a thread owns 4 consecutive k for the whole batch tile (128 accumulators); the dz slice sits in shared memory as
 // [n][32 b] and is read with warp-broadcast 16-byte loads; weights stream through with coalesced float4 loads.
 __global__ void __launch_bounds__(128) linear_dgrad_f32_kernel(const float* __restrict__ dz, const float* __restrict__ w, float* dacc,
-                                                              int B, int N, int K, int lddz, int ldw, int ldd, int nc) {
+                                                              int B, int N, int K, int lddz, int ldw, int ldd, int nc,
+                                                              const Det det) {
   pdl_trigger();
   pdl_wait();
   extern __shared__ __align__(16) float s_dz[];                  // [nc][32]
@@ -1059,12 +1170,23 @@ __global__ void __launch_bounds__(128) linear_dgrad_f32_kernel(const float* __re
   for (int bp = 0; bp < 16; ++bp)
 #pragma unroll
     for (int k = 0; k < 4; ++k) unpack2(acc[bp][k], a[2 * bp][k], a[2 * bp + 1][k]);
+  // N slices add in slice order (blockIdx.y) behind a turn counter: the same sum every run
+  uint32_t* turn = det.ctr + DET_TURN_BASE + blockIdx.z * gridDim.x + blockIdx.x;
+  if (gridDim.y > 1) {
+    if (threadIdx.x == 0) turn_wait(turn, blockIdx.y);
+    __syncthreads();
+  }
 #pragma unroll
   for (int b = 0; b < 32; ++b)
     if (b0 + b < B)
       asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dacc + (long long)(b0 + b) * ldd + k0), "f"(a[b][0]),
                    "f"(a[b][1]), "f"(a[b][2]), "f"(a[b][3])
                    : "memory");
+  if (gridDim.y > 1) {
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) turn_pass(turn, blockIdx.y, gridDim.y);
+  }
 }
 
 // g[n][k] = sum_b dz[b][n] * x[b][k]  (K = batch: the weight gradient is written exactly once, so the optimizer step
@@ -1183,12 +1305,14 @@ __global__ void __launch_bounds__(256) clip_scale_kernel(float4* g, long long n4
 // ============================================================================ cross-entropy forward + backward
 // one warp per sample: loss_sum += -log softmax[label] / B; dlogits = (softmax - onehot) / B  (fp32, ld = ldd)
 __global__ void ce_fwd_bwd_kernel(const float* logits, const long long* labels, float* dlogits, float* loss_sum,
-                                  int* nan_flag, int B, int C, int ldd) {
+                                  int* nan_flag, int B, int C, int ldd, const Det det) {
   pdl_trigger();
   pdl_wait();
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  if (warp >= B) return;
+  __shared__ float s_loss[32];
+  float loss_v = 0.f;
+  if (warp < B) {
   const float* row = logits + (long long)warp * C;
   float mx = -INFINITY;
   for (int c = lane; c < C; c += 32) mx = fmaxf(mx, row[c]);
@@ -1206,8 +1330,19 @@ __global__ void ce_fwd_bwd_kernel(const float* logits, const long long* labels, 
   }
   if (lane == 0) {
     const float loss = lse - row[lab];
-    atomicAdd(loss_sum, loss * invB);
+    loss_v = loss * invB;
     if (loss != loss) *nan_flag = 1;
+  }
+  }
+  if (lane == 0) s_loss[threadIdx.x >> 5] = loss_v;
+  __syncthreads();
+  if (threadIdx.x == 0) {                 // rows in order (blocks behind a turn counter): the same loss every run
+    uint32_t* turn = det.ctr + DET_TURN_BASE;
+    if (gridDim.x > 1) turn_wait(turn, blockIdx.x);
+    float sum = *loss_sum;
+    for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) sum += s_loss[w];
+    *loss_sum = sum;
+    if (gridDim.x > 1) turn_pass(turn, blockIdx.x, gridDim.x);
   }
 }
 
@@ -1325,7 +1460,7 @@ __global__ void __launch_bounds__(512) fedavg_kernel(float4* out, uint2* out_bf1
   }
 }
 
-static inline int grid_for(long long work, int block, int max_blocks = 148 * 8) {
+static inline int grid_for(long long work, int block, int max_blocks = 132 * 8) {
   long long g = (work + block - 1) / block;
   if (g < 1) g = 1;
   if (g > max_blocks) g = max_blocks;
@@ -1345,6 +1480,7 @@ int slb_preload_elementwise() {
   using bf = __nv_bfloat16;
   cudaFuncAttributes a;
   int bad = 0;
+  bad += slb_det(nullptr).part != nullptr ? 0 : 1;                // reduction scratch, before any graph capture
 #define SLB_PRELOAD(k) bad += (cudaFuncGetAttributes(&a, k) != cudaSuccess)
 #define SLB_PRELOAD_T(T) \
   { auto k = bn_relu_pool_fwd_kernel<T>; SLB_PRELOAD(k); } \
@@ -1418,7 +1554,7 @@ static int bn_fwd_t(const void* y, const float* sum, const float* sumsq, const f
                       save_mean, save_invstd, reinterpret_cast<T*>(out), P, C, H, W, relu, pool, momentum, eps,
                       update_running, identity, ticket, flag, seq, hint};
   const long long work = (pool ? (long long)P / 4 : P) * (C / 8);
-  launch_k(bn_relu_pool_fwd_kernel<T>, grid_for(work, 256, 148 * 4), 256, 2 * C * sizeof(float), st, p);
+  launch_k(bn_relu_pool_fwd_kernel<T>, grid_for(work, 256, 132 * 4), 256, 2 * C * sizeof(float), st, p);
   return last_err();
 }
 extern "C" {
@@ -1452,17 +1588,19 @@ static int bn_bwd_t(const void* dout, const void* y, const float* gamma, const f
   const bool skip_reduce = identity == 2;
   if (skip_reduce) { identity = 0; grid_bar = nullptr; }
   BnBwdParams<T> p = {reinterpret_cast<const T*>(dout), reinterpret_cast<const T*>(y), gamma, beta,
-                      save_mean, save_invstd, dgamma, dbeta, reinterpret_cast<T*>(dy), P, C, H, W, relu, pool, identity};
+                      save_mean, save_invstd, dgamma, dbeta, reinterpret_cast<T*>(dy), P, C, H, W, relu, pool, identity,
+                      slb_det(st)};
   const int tx = C / 8;
   const int ty = tx >= 256 ? 1 : 256 / tx;
   dim3 block(tx, ty);
   const long long outP = pool ? (long long)P / 4 : P;
-  const int grid = grid_for(outP, ty, 148 * 2);
+  const int grid = grid_for(outP, ty, 132 * 2);
+  if (p.det.part == nullptr || (long long)grid * 2 * C > p.det.cap) return -30;
   if (grid_bar != nullptr && !identity) {          // one launch: reduce -> grid barrier -> apply
     // the software barrier needs every block co-resident: cap the grid at (SMs - 4) x measured occupancy
     static int cap[2] = {0, 0};
     if (cap[pool ? 1 : 0] == 0) {
-      int per_sm = 0, dev = 0, sms = 148;
+      int per_sm = 0, dev = 0, sms = 132;
       cudaGetDevice(&dev);
       cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
       if (pool) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bn_bwd_fused_kernel<true, T>, 256, 2 * 2048 * sizeof(float));
@@ -1505,23 +1643,27 @@ int slb_conv_finalize(const float* acc, const float* bias, void* y, float* sum, 
                       cudaStream_t st) {
   if (C % 8) return -1;
   const int tx = C / 8, ty = tx >= 256 ? 1 : 256 / tx;
+  const Det det = slb_det(st);
+  if (det.part == nullptr || (long long)grid_for(P, ty, 132 * 2) * 2 * C > det.cap) return -30;
   if (dtype == 1)
-    launch_k(conv_finalize_kernel<float>, grid_for(P, ty, 148 * 2), dim3(tx, ty), 2 * C * sizeof(float), st, acc, bias,
-             reinterpret_cast<float*>(y), sum, sumsq, P, C);
+    launch_k(conv_finalize_kernel<float>, grid_for(P, ty, 132 * 2), dim3(tx, ty), 2 * C * sizeof(float), st, acc, bias,
+             reinterpret_cast<float*>(y), sum, sumsq, P, C, det);
   else
-    launch_k(conv_finalize_kernel<__nv_bfloat16>, grid_for(P, ty, 148 * 2), dim3(tx, ty), 2 * C * sizeof(float), st, acc, bias,
-             reinterpret_cast<__nv_bfloat16*>(y), sum, sumsq, P, C);
+    launch_k(conv_finalize_kernel<__nv_bfloat16>, grid_for(P, ty, 132 * 2), dim3(tx, ty), 2 * C * sizeof(float), st, acc, bias,
+             reinterpret_cast<__nv_bfloat16*>(y), sum, sumsq, P, C, det);
   return last_err();
 }
 int slb_col_stats(const void* y, float* sum, float* sumsq, long long P, int C, int dtype, cudaStream_t st) {
   if (C % 8) return -1;
   const int tx = C / 8, ty = tx >= 256 ? 1 : 256 / tx;
+  const Det det = slb_det(st);
+  if (det.part == nullptr || (long long)grid_for(P, ty, 132 * 2) * 2 * C > det.cap) return -30;
   if (dtype == 1)
-    launch_k(col_stats_kernel<float>, grid_for(P, ty, 148 * 2), dim3(tx, ty), 2 * C * sizeof(float), st,
-             reinterpret_cast<const float*>(y), sum, sumsq, P, C);
+    launch_k(col_stats_kernel<float>, grid_for(P, ty, 132 * 2), dim3(tx, ty), 2 * C * sizeof(float), st,
+             reinterpret_cast<const float*>(y), sum, sumsq, P, C, det);
   else
-    launch_k(col_stats_kernel<__nv_bfloat16>, grid_for(P, ty, 148 * 2), dim3(tx, ty), 2 * C * sizeof(float), st,
-             reinterpret_cast<const __nv_bfloat16*>(y), sum, sumsq, P, C);
+    launch_k(col_stats_kernel<__nv_bfloat16>, grid_for(P, ty, 132 * 2), dim3(tx, ty), 2 * C * sizeof(float), st,
+             reinterpret_cast<const __nv_bfloat16*>(y), sum, sumsq, P, C, det);
   return last_err();
 }
 
@@ -1532,10 +1674,12 @@ static int small_fwd_t(const float* x, const float* w, const float* bias, void* 
   const long long P = (long long)B * H * W;
   const int grid = static_cast<int>((P + 127) / 128);
   T* yy = reinterpret_cast<T*>(y);
-  if (Cin == 3 && Cout == 64) launch_k(conv3x3_small_fwd_kernel<3, 64, T>, grid, 128, 0, st, x, w, bias, yy, sum, sumsq, B, H, W);
-  else if (Cin == 3 && Cout == 32) launch_k(conv3x3_small_fwd_kernel<3, 32, T>, grid, 128, 0, st, x, w, bias, yy, sum, sumsq, B, H, W);
-  else if (Cin == 1 && Cout == 64) launch_k(conv3x3_small_fwd_kernel<1, 64, T>, grid, 128, 0, st, x, w, bias, yy, sum, sumsq, B, H, W);
-  else if (Cin == 1 && Cout == 32) launch_k(conv3x3_small_fwd_kernel<1, 32, T>, grid, 128, 0, st, x, w, bias, yy, sum, sumsq, B, H, W);
+  const Det det = slb_det(st);
+  if (det.part == nullptr || (long long)grid * 2 * Cout > det.cap) return -30;
+  if (Cin == 3 && Cout == 64) launch_k(conv3x3_small_fwd_kernel<3, 64, T>, grid, 128, 0, st, x, w, bias, yy, sum, sumsq, B, H, W, det);
+  else if (Cin == 3 && Cout == 32) launch_k(conv3x3_small_fwd_kernel<3, 32, T>, grid, 128, 0, st, x, w, bias, yy, sum, sumsq, B, H, W, det);
+  else if (Cin == 1 && Cout == 64) launch_k(conv3x3_small_fwd_kernel<1, 64, T>, grid, 128, 0, st, x, w, bias, yy, sum, sumsq, B, H, W, det);
+  else if (Cin == 1 && Cout == 32) launch_k(conv3x3_small_fwd_kernel<1, 32, T>, grid, 128, 0, st, x, w, bias, yy, sum, sumsq, B, H, W, det);
   else return -2;
   return last_err();
 }
@@ -1554,14 +1698,16 @@ static int small_wgrad_t(const float* x, const void* dy, float* dw, int B, int C
   const long long chunks = ((long long)B * H * W + 127) / 128;
   const int grid = static_cast<int>(chunks < 296 ? chunks : 296);   // 2 CTAs per SM: the staging phase of one hides behind the FMAs of the other
   const T* d = reinterpret_cast<const T*>(dy);
+  const Det det = slb_det(st);
+  if (det.part == nullptr || (long long)grid * Cout * 9 * Cin > det.cap) return -30;
   if (Cin == 3) {
     static bool done3 = false;
     if (!done3) { cudaFuncSetAttribute(conv3x3_small_wgrad_kernel<3, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024); done3 = true; }
-    launch_k(conv3x3_small_wgrad_kernel<3, T>, grid, 256, smem, st, x, d, dw, B, H, W, Cout);
+    launch_k(conv3x3_small_wgrad_kernel<3, T>, grid, 256, smem, st, x, d, dw, B, H, W, Cout, det);
   } else if (Cin == 1) {
     static bool done1 = false;
     if (!done1) { cudaFuncSetAttribute(conv3x3_small_wgrad_kernel<1, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024); done1 = true; }
-    launch_k(conv3x3_small_wgrad_kernel<1, T>, grid, 256, smem, st, x, d, dw, B, H, W, Cout);
+    launch_k(conv3x3_small_wgrad_kernel<1, T>, grid, 256, smem, st, x, d, dw, B, H, W, Cout, det);
   } else return -2;
   return last_err();
 }
@@ -1619,7 +1765,10 @@ int slb_linear_fwd_f32(const float* x, const float* w, float* acc, int B, int N,
   dim3 grid(fgroups, (K + kc - 1) / kc, (B + 31) / 32);
   static bool attr = false;
   if (!attr) { cudaFuncSetAttribute(linear_fwd_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 32 * 128 * 4); attr = true; }
-  launch_k(linear_fwd_f32_kernel, grid, dim3(256), (size_t)4 * 32 * 128 * sizeof(float), st, x, w, acc, B, N, K, ldx, ldw, lda, kc);
+  const Det det = slb_det(st);
+  if (det.part == nullptr || (long long)grid.x * grid.z > DET_COUNTERS - DET_TURN_BASE) return -30;
+  launch_k(linear_fwd_f32_kernel, grid, dim3(256), (size_t)4 * 32 * 128 * sizeof(float), st, x, w, acc, B, N, K, ldx, ldw, lda, kc,
+           det);
   return last_err();
 }
 int slb_linear_dgrad_f32(const float* dz, const float* w, float* dacc, int B, int N, int K, int lddz, int ldw, int ldd,
@@ -1633,7 +1782,9 @@ int slb_linear_dgrad_f32(const float* dz, const float* w, float* dacc, int B, in
   const size_t smem = (size_t)nc * 32 * sizeof(float) + (size_t)6 * 4 * threads * 16;      // dz slice + per-thread weight ring
   static bool attr = false;
   if (!attr) { cudaFuncSetAttribute(linear_dgrad_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024); attr = true; }
-  launch_k(linear_dgrad_f32_kernel, grid, dim3(threads), smem, st, dz, w, dacc, B, N, K, lddz, ldw, ldd, nc);
+  const Det det = slb_det(st);
+  if (det.part == nullptr || (long long)grid.x * grid.z > DET_COUNTERS - DET_TURN_BASE) return -30;
+  launch_k(linear_dgrad_f32_kernel, grid, dim3(threads), smem, st, dz, w, dacc, B, N, K, lddz, ldw, ldd, nc, det);
   return last_err();
 }
 // mode 0: G = g, 1: G += g, 2: fused SGD-momentum on (P, M) [+ bias rows].  Batches > 32 are looped here (mode 2 needs B <= 32).
@@ -1654,23 +1805,25 @@ int slb_linear_wgrad_f32(const float* dz, const float* x, float* G, float* P, fl
 }
 int slb_sumsq(const float* g, long long n, float* out, cudaStream_t st) {
   if (n % 4) return -1;
-  launch_k(sumsq_kernel, grid_for(n / 4, 256, 148 * 8), 256, 0, st, reinterpret_cast<const float4*>(g), n / 4, out);
+  launch_k(sumsq_kernel, grid_for(n / 4, 256, 132 * 8), 256, 0, st, reinterpret_cast<const float4*>(g), n / 4, out);
   return last_err();
 }
 int slb_clip_scale(float* g, long long n, const float* sumsq, float max_norm, cudaStream_t st) {
   if (n % 4) return -1;
-  launch_k(clip_scale_kernel, grid_for(n / 4, 256, 148 * 8), 256, 0, st, reinterpret_cast<float4*>(g), n / 4, sumsq, max_norm);
+  launch_k(clip_scale_kernel, grid_for(n / 4, 256, 132 * 8), 256, 0, st, reinterpret_cast<float4*>(g), n / 4, sumsq, max_norm);
   return last_err();
 }
 
 int slb_ce_fwd_bwd(const float* logits, const long long* labels, float* dlogits, float* loss_sum, int* nan_flag, int B, int C,
                    int ldd, cudaStream_t st) {
-  launch_k(ce_fwd_bwd_kernel, (B * 32 + 127) / 128, 128, 0, st, logits, labels, dlogits, loss_sum, nan_flag, B, C, ldd);
+  const Det det = slb_det(st);
+  if (det.part == nullptr) return -30;
+  launch_k(ce_fwd_bwd_kernel, (B * 32 + 127) / 128, 128, 0, st, logits, labels, dlogits, loss_sum, nan_flag, B, C, ldd, det);
   return last_err();
 }
 int slb_sgd_momentum(float* p, float* g, float* m, void* p_bf16, long long n, float lr, float mu, int first_step, cudaStream_t st) {
   if (n % 4) return -1;
-  launch_k(sgd_momentum_kernel, grid_for(n / 4, 256, 148 * 16), 256, 0, st, reinterpret_cast<float4*>(p), reinterpret_cast<float4*>(g),
+  launch_k(sgd_momentum_kernel, grid_for(n / 4, 256, 132 * 16), 256, 0, st, reinterpret_cast<float4*>(p), reinterpret_cast<float4*>(g),
                                                                      reinterpret_cast<float4*>(m), reinterpret_cast<uint2*>(p_bf16),
                                                                      n / 4, lr, mu, first_step);
   return last_err();
@@ -1678,7 +1831,7 @@ int slb_sgd_momentum(float* p, float* g, float* m, void* p_bf16, long long n, fl
 int slb_adamw(float* p, float* g, float* m, float* v, void* p_bf16, long long n, float lr, float b1, float b2, float eps, float wd,
               float bc1, float bc2, const uint32_t* step_ptr, cudaStream_t st) {
   if (n % 4) return -1;
-  launch_k(adamw_kernel, grid_for(n / 4, 256, 148 * 16), 256, 0, st, reinterpret_cast<float4*>(p), reinterpret_cast<float4*>(g),
+  launch_k(adamw_kernel, grid_for(n / 4, 256, 132 * 16), 256, 0, st, reinterpret_cast<float4*>(p), reinterpret_cast<float4*>(g),
                                                               reinterpret_cast<float4*>(m), reinterpret_cast<float4*>(v),
                                                               reinterpret_cast<uint2*>(p_bf16), n / 4, lr, b1, b2, eps, wd, bc1, bc2, step_ptr);
   return last_err();
@@ -1687,13 +1840,13 @@ int slb_image_batch(const void* data, const long long* idx, const int* dx, const
                     int C, int H, int W, const float* mean3, const float* std3, cudaStream_t st) {
   if (C < 1 || C > 3) return -1;
   const long long total = (long long)B * C * H * W;
-  launch_k(image_batch_kernel, grid_for(total, 256, 148 * 8), 256, 0, st, reinterpret_cast<const uint8_t*>(data), idx, dx, dy,
+  launch_k(image_batch_kernel, grid_for(total, 256, 132 * 8), 256, 0, st, reinterpret_cast<const uint8_t*>(data), idx, dx, dy,
            flip, out, B, C, H, W, mean3[0], mean3[1], mean3[2], std3[0], std3[1], std3[2]);
   return last_err();
 }
 int slb_cast_f32_bf16(const float* x, void* y, long long n, cudaStream_t st) {
   if (n % 4) return -1;
-  launch_k(cast_f32_bf16_kernel, grid_for(n / 4, 256, 148 * 16), 256, 0, st, reinterpret_cast<const float4*>(x), reinterpret_cast<uint2*>(y), n / 4);
+  launch_k(cast_f32_bf16_kernel, grid_for(n / 4, 256, 132 * 16), 256, 0, st, reinterpret_cast<const float4*>(x), reinterpret_cast<uint2*>(y), n / 4);
   return last_err();
 }
 // srcs: host array of nsrc device pointers (local or peer-mapped), coefs: host array
@@ -1702,7 +1855,7 @@ int slb_fedavg(float* out, void* out_bf16, const float* const* srcs, const float
   FedAvgParams p;
   for (int i = 0; i < 16; ++i) { p.src[i] = i < nsrc ? srcs[i] : nullptr; p.coef[i] = i < nsrc ? coefs[i] : 0.f; }
   p.nsrc = nsrc;
-  launch_k(fedavg_kernel, grid_for(n / 4, 512, 148 * 4), 512, 0, st, reinterpret_cast<float4*>(out), reinterpret_cast<uint2*>(out_bf16), p, n / 4);
+  launch_k(fedavg_kernel, grid_for(n / 4, 512, 132 * 4), 512, 0, st, reinterpret_cast<float4*>(out), reinterpret_cast<uint2*>(out_bf16), p, n / 4);
   return last_err();
 }
 

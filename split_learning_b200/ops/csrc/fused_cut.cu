@@ -1,17 +1,17 @@
 // Cut-tail forward kernel (SURVEY §2.7 G1+G4+G5+G13, §7.4 "hard part" #1):
 //
-//   conv3x3 (tcgen05 implicit GEMM, accumulators stay in TMEM)
+//   conv3x3 (wgmma implicit GEMM, the accumulator tile then stays in shared memory)
 //     -> per-channel batch statistics from the accumulators (+bias)
-//     -> grid-wide barrier (cooperative persistent launch, every tile resident in TMEM)
-//     -> BatchNorm(train) + ReLU + 2x2 MaxPool applied straight out of TMEM
+//     -> grid-wide barrier (persistent launch, every tile resident in shared memory)
+//     -> BatchNorm(train) + ReLU + 2x2 MaxPool applied straight out of shared memory
 //     -> bf16 tiles stored into the NEXT stage's mailbox slot (local or NVLink-peer pointer)
 //     -> last CTA publishes the slot flag with st.release.sys.
 //
 // The pre-BN activation never touches HBM on the forward-only pass of a recomputing stage:
 // the only global traffic is x, w, 2*C floats of statistics and the (pooled) cut payload that
-// crosses the link.  One persistent CTA per SM; CTA c owns tiles c, c+G, ... (<= 512/BLOCK_N
-// accumulators of 128 x BLOCK_N fp32 fit the 512 TMEM columns).
-#include "sm100.cuh"
+// crosses the link.  One persistent CTA per SM; CTA c owns tiles c, c+G, ... (at most MAX_TILES:
+// the fp32 accumulators of the last tile re-use the pipeline buffers, earlier ones have their own slot).
+#include "sm90.cuh"
 
 #include <cooperative_groups.h>
 
@@ -40,6 +40,7 @@ struct FusedCutParams {
   uint32_t* flag;
   uint32_t* seq;
   uint32_t* hint;
+  Det det;                  // reproducible cross-CTA sum of the batch statistics
 };
 
 template <int BLOCK_N>
@@ -47,13 +48,22 @@ struct FusedSmem {
   static constexpr int A_BYTES = 128 * 128;
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BLOCK_N >= 256) ? 4 : (BLOCK_N >= 128 ? 5 : 6);
+  static constexpr int STAGES = (BLOCK_N >= 128) ? 4 : 6;
   static constexpr int TILE_BYTES = STAGES * STAGE_BYTES;
-  static constexpr int MAX_TILES = 512 / BLOCK_N;
+  // after the MMAs the ring holds the pooling stage tile [128][33] and the last tile's fp32 accumulators [128][ACC_LD]
+  static constexpr int ACC_OFF = 17 * 1024;
+  static constexpr int ACC_LD = BLOCK_N + 4;
+  static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
+  static constexpr int MAX_TILES = BLOCK_N <= 128 ? 2 : 1;
   static constexpr int TAIL_BYTES = 4096;
   static constexpr int TR_BYTES = 4 * 32 * 33 * 4;   // warp-private transpose tiles of the statistics reduction
-  static constexpr int TOTAL = TILE_BYTES + TAIL_BYTES + TR_BYTES + 1024;
-  static_assert(TILE_BYTES >= 128 * 33 * 4, "staging tile must fit in the pipeline buffers");
+  static constexpr int EXTRA_OFF = TILE_BYTES + TAIL_BYTES + TR_BYTES;   // accumulators of the earlier tiles
+  static constexpr int TOTAL = EXTRA_OFF + (MAX_TILES - 1) * ACC_BYTES + 1024;
+  static constexpr int TOT_OFF = ACC_OFF + ACC_BYTES;   // per-CTA statistics [2][N], N <= MAX_N, behind the last tile
+  static constexpr int MAX_N = 512;
+  static_assert(TOT_OFF + 2 * MAX_N * 4 <= TILE_BYTES, "statistics must fit in the pipeline buffers");
+  static_assert(128 * 33 * 4 <= ACC_OFF, "staging tile must fit in front of the accumulator tile");
+  static_assert(ACC_OFF + 128 * ACC_LD * 4 <= TILE_BYTES, "accumulator tile must fit in the pipeline buffers");
 };
 
 __device__ __forceinline__ float warp_col_reduce32f(float (&v)[32]) {
@@ -72,7 +82,7 @@ __device__ __forceinline__ float warp_col_reduce32f(float (&v)[32]) {
 }
 
 template <int BLOCK_N, typename T>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(288, 1)
 conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                        const FusedCutParams p) {
   using L = FusedSmem<BLOCK_N>;
@@ -84,19 +94,20 @@ conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES);
   uint64_t* empty_bar = full_bar + L::STAGES;
-  uint64_t* accum_bar = empty_bar + L::STAGES;                  // [MAX_TILES]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + L::MAX_TILES);
-  float* s_scale = reinterpret_cast<float*>(tmem_slot + 4);     // [BLOCK_N]
+  float* s_scale = reinterpret_cast<float*>(empty_bar + L::STAGES);   // [BLOCK_N]
   float* s_shift = s_scale + BLOCK_N;                           // [BLOCK_N]
   float* s_bias = s_shift + BLOCK_N;                            // [BLOCK_N] bias of the current tile's columns
   float* s_tr_all = reinterpret_cast<float*>(smem + L::TILE_BYTES + L::TAIL_BYTES);   // 4 x [32][33]
   float* s_stage = reinterpret_cast<float*>(smem);              // [128][33] fp32, reuses the pipeline buffers
+  float* s_acc = reinterpret_cast<float*>(smem + L::ACC_OFF);   // [128][ACC_LD] accumulators of this CTA's last tile
+  float* s_extra = reinterpret_cast<float*>(smem + L::EXTRA_OFF); // [MAX_TILES - 1][128][ACC_LD] the earlier tiles
 
   const int warp = threadIdx.x >> 5;
   const int G = gridDim.x;
   const int total_tiles = p.tiles_m * p.tiles_n;
   int my_tiles = 0;
   for (int t = blockIdx.x; t < total_tiles; t += G) ++my_tiles;
+  auto tile_acc = [&](int j) { return j == my_tiles - 1 ? s_acc : s_extra + j * (L::ACC_BYTES / 4); };
   const int k_iters = 9 * (p.C / KE);
 
   if (threadIdx.x == 0) {
@@ -104,18 +115,13 @@ conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < L::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);                 // one arrival per consumer warpgroup
     }
-    for (int j = 0; j < L::MAX_TILES; ++j) mbar_init(&accum_bar[j], 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ============================== TMA producer ==============================
     if (elect_one()) {
       int stage = 0;
@@ -138,35 +144,27 @@ conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================== MMA issuer ==============================
-    const uint32_t idesc = umma_idesc(128, BLOCK_N, false, false, OT::FMT);
+  } else {
+    // ============================== two wgmma warpgroups ==============================
     int stage = 0;
     uint32_t phase = 0;
     for (int j = 0; j < my_tiles; ++j) {
-      for (int it = 0; it < k_iters; ++it) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_base = smem_u32(smem + stage * L::STAGE_BYTES);
-          const uint32_t b_base = a_base + L::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_issue<T>(tmem_base + j * BLOCK_N, umma_desc_sw128(a_base + k * 32, 16, 1024),
-                          umma_desc_sw128(b_base + k * 32, 16, 1024), idesc, (it | k) != 0 ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (it == k_iters - 1) umma_commit(&accum_bar[j]);
-        }
-        __syncwarp();
-        if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
-      }
+      float acc[BLOCK_N / 2];
+      wg_mainloop<T, BLOCK_N>(smem, nullptr, L::STAGE_BYTES, L::A_BYTES, L::STAGES, full_bar, empty_bar, k_iters, 0, 0, acc,
+                              stage, phase);
+      if (j == my_tiles - 1) asm volatile("bar.sync 2, 256;" ::: "memory");   // no MMA reads the ring any more
+      wg_store_acc<BLOCK_N>(tile_acc(j) + (threadIdx.x >> 7) * 64 * L::ACC_LD, L::ACC_LD, acc);
     }
-  } else {
+    asm volatile("bar.sync 2, 256;" ::: "memory");
+  }
+  if (warp < 4) {
     // ============================== epilogue ==============================
-    const int q = warp & 3;
-    const int lrow = q * 32 + lane_id();            // row inside the tile == TMEM lane
-    const int et = (warp - 2) * 32 + lane_id();
+    const int q = warp;
+    const int lrow = q * 32 + lane_id();            // row inside the tile
+    const int et = threadIdx.x;
     const uint32_t gen = ld_acquire_gpu(p.grid_bar + 1);
+    float* s_tot = reinterpret_cast<float*>(smem + L::TOT_OFF);     // this CTA's column sums, all its tiles
+    for (int i = et; i < 2 * p.N; i += 128) s_tot[i] = 0.f;
 
     // ---- phase 1: statistics (and optional y) from the accumulators ----
     for (int j = 0; j < my_tiles; ++j) {
@@ -175,16 +173,13 @@ conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       const int row = m0 + lrow;
       const bool row_ok = row < p.M;
       asm volatile("bar.sync 1, 128;");                 // previous tile's readers are done with s_bias
-      for (int i = et; i < BLOCK_N; i += 128) s_bias[i] = __ldg(p.bias + n0 + i);   // overlaps the tile's MMAs
+      for (int i = et; i < BLOCK_N; i += 128) s_bias[i] = __ldg(p.bias + n0 + i);
       asm volatile("bar.sync 1, 128;");
-      mbar_wait(&accum_bar[j], 0);
-      tc_fence_after();
-      float* s_tr = s_tr_all + (warp - 2) * (32 * 33);
+      float* s_tr = s_tr_all + warp * (32 * 33);
 #pragma unroll 1
       for (int c = 0; c < BLOCK_N; c += 32) {
         uint32_t v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + j * BLOCK_N + c, v);
-        tmem_ld_wait();
+        acc_ld32(tile_acc(j), L::ACC_LD, lrow, c, v);
         float s1[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) s1[i] = row_ok ? __uint_as_float(v[i]) + s_bias[c + i] : 0.f;
@@ -202,10 +197,14 @@ conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           c2 = fmaf(x, x, c2);
         }
         __syncwarp();
-        atomicAdd(p.sum + n0 + c + lane_id(), c1);
-        atomicAdd(p.sumsq + n0 + c + lane_id(), c2);
+        for (int w = 0; w < 4; ++w) {                       // warps in order: a reproducible sum
+          if (warp == w) { s_tot[n0 + c + lane_id()] += c1; s_tot[p.N + n0 + c + lane_id()] += c2; }
+          asm volatile("bar.sync 1, 128;" ::: "memory");
+        }
       }
     }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    det_commit<1>(p.det, 0, blockIdx.x, G, s_tot, 2 * p.N, p.sum, p.N, p.sumsq, et, 128);   // CTA order
     // ---- grid barrier: every CTA has contributed its partial sums ----
     asm volatile("bar.sync 1, 128;");
     if (et == 0) {
@@ -215,12 +214,12 @@ conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       uint32_t spins = 0;
       while (static_cast<int32_t>(ld_acquire_gpu(p.grid_bar) - target) < 0) {
         __nanosleep(32);
-        if (++spins > (1u << 26)) { printf("slb: fused cut grid barrier timeout\n"); __trap(); }
+        if (++spins > (1u << 26)) __trap();                         // no printf: see mbar_wait
       }
     }
     asm volatile("bar.sync 1, 128;");
 
-    // ---- phase 2: BN + ReLU (+pool) out of TMEM, store to the mailbox ----
+    // ---- phase 2: BN + ReLU (+pool) out of the accumulator tile, store to the mailbox ----
     const float invM = 1.f / static_cast<float>(p.M);
     const int OW = p.W >> 1, OH = p.H >> 1;
     for (int j = 0; j < my_tiles; ++j) {
@@ -253,8 +252,7 @@ conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 #pragma unroll 1
       for (int c = 0; c < BLOCK_N; c += 32) {
         uint32_t v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + j * BLOCK_N + c, v);
-        tmem_ld_wait();
+        acc_ld32(tile_acc(j), L::ACC_LD, lrow, c, v);
         float z[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
@@ -315,12 +313,6 @@ conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
 }
 
 typedef CUresult (*PFN_encodeTiled2)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -365,11 +357,11 @@ static int launch_fused(const CUtensorMap& a, const CUtensorMap& b, const FusedC
     if (e != cudaSuccess) return -static_cast<int>(e) - 1000;
     attr_done = true;
   }
-  // Plain (non-cooperative) launch with grid <= #SMs and one CTA per SM (152+ KB of smem each): co-residency of the
+  // Plain (non-cooperative) launch with grid <= #SMs and one CTA per SM (150+ KB of smem each): co-residency of the
   // software grid barrier holds as soon as every SM has drained whatever independent kernel of another stream it was
   // running.  cudaLaunchCooperativeKernel is NOT used: the driver would not start it while any other kernel of the
   // context is resident — e.g. the next stage's flag-wait kernel that only this kernel can release (observed dead-lock).
-  k<<<dim3(grid), dim3(192), FusedSmem<BN>::TOTAL, st>>>(a, b, p);
+  k<<<dim3(grid), dim3(288), FusedSmem<BN>::TOTAL, st>>>(a, b, p);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : -static_cast<int>(e) - 2000;
 }
@@ -391,7 +383,7 @@ int slb_preload_fused() {
   return bad;
 }
 
-// Fused cut-tail forward.  x [B,H,W,Cin], w [Cout][3][3][Cin], y_opt / out: bf16 (dtype 0) or fp32 (dtype 1, kind::tf32).
+// Fused cut-tail forward.  x [B,H,W,Cin], w [Cout][3][3][Cin], y_opt / out: bf16 (dtype 0) or fp32 (dtype 1, wgmma tf32).
 // `out` may be a peer pointer.
 // `grid_bar`: 4 zero-initialised uint32 owned by this call site.  sum/sumsq: zeroed by the caller.
 int slb_conv_bn_act_p2p(const void* x, const void* w, const float* bias, const float* gamma, const float* beta,
@@ -415,7 +407,7 @@ int slb_conv_bn_act_p2p(const void* x, const void* w, const float* bias, const f
   // waiting for *this* kernel's flag.  With spare SMs every CTA of the software grid barrier can always become resident.
   const int usable = num_sms > 8 ? num_sms - 4 : num_sms;
   int grid = total < usable ? total : usable;
-  if ((total + grid - 1) / grid > 512 / bn) return -15;          // accumulators would not fit in TMEM
+  if ((total + grid - 1) / grid > (bn <= 128 ? 2 : 1)) return -15;   // FusedSmem<bn>::MAX_TILES
   CUtensorMap ta, tbm;
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
@@ -436,6 +428,8 @@ int slb_conv_bn_act_p2p(const void* x, const void* w, const float* bias, const f
   p.y = y_opt; p.out = out;
   p.relu = relu; p.pool = pool; p.momentum = momentum; p.eps = eps; p.update_running = update_running;
   p.grid_bar = grid_bar; p.flag = flag; p.seq = seq; p.hint = hint;
+  p.det = slb_det(st);
+  if (p.det.part == nullptr || Cout > 512 || (long long)grid * 2 * Cout > p.det.cap) return -30;
   if (dtype == 1) {
     switch (bn) {
       case 64: return launch_fused<64, float>(ta, tbm, p, grid, st);

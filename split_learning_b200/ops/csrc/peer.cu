@@ -4,6 +4,9 @@
 // without a device round trip.  (SURVEY §5 "Distributed communication backend".)
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "sm90.cuh"
+#include <stdint.h>
 #include <string.h>
 
 extern "C" {
@@ -32,10 +35,14 @@ int slb_stream_create(void** out, int high) {
   cudaStream_t s;
   cudaError_t e = cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, high ? greatest : least);
   if (e != cudaSuccess) return -static_cast<int>(e);
+  slb::slb_det(s);                        // its reduction scratch, now rather than inside a graph capture
   *out = s;
   return 0;
 }
-int slb_stream_destroy(void* s) { return -static_cast<int>(cudaStreamDestroy(static_cast<cudaStream_t>(s))); }
+int slb_stream_destroy(void* s) {
+  slb::slb_det_release(static_cast<cudaStream_t>(s));
+  return -static_cast<int>(cudaStreamDestroy(static_cast<cudaStream_t>(s)));
+}
 
 int slb_ipc_get_handle(void* p, uint8_t* out64) {
   cudaIpcMemHandle_t h;

@@ -11,7 +11,7 @@
 // A ticket is claimed by exactly one replica (the atomic), in FIFO order, and names the origin (whose outbox slot holds the
 // payload and whose gradient mailbox receives dX) — the reference's `trace[-1]`.  The claim result goes to mapped pinned
 // host memory: the host picks the program (origin, slot) to enqueue, which is also how it learns that the round is drained.
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace slb {
 

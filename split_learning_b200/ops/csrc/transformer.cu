@@ -1,10 +1,10 @@
 // Encoder-block kernels for the token-model families (KWT / ViT / BERT; SURVEY §2.7 G11):
 //
 //   attn_fwd_kernel / attn_bwd_kernel
-//       dense softmax attention for S <= 128, one CTA per (batch, head), everything on tcgen05:
-//       S = Q K^T and O = P V (forward), S / dP / dV / dQ / dK (backward) are single-tile UMMAs whose operands are
-//       TMA boxes of the *packed* projection output (no head split / transpose copies exist); the softmax runs on
-//       the TMEM accumulator with one thread per query row (tcgen05.ld 32x32b -> no cross-thread reduction) and
+//       dense softmax attention for S <= 128, one CTA (one warpgroup) per (batch, head), everything on wgmma:
+//       S = Q K^T and O = P V (forward), S / dP / dV / dQ / dK (backward) are 128-row tiles computed as two 64-row
+//       wgmma halves whose operands are TMA boxes of the *packed* projection output (no head split / transpose
+//       copies exist); the softmax runs on the register accumulators (a row spans the 4 threads of a quad) and
 //       writes P / dS back to shared memory in the 128B-swizzled layout, so the same bytes serve as the K-major A
 //       operand (P V, dS K) and as the MN-major A operand (P^T dO, dS^T Q).  Probability dropout is a counter
 //       hash, regenerated in the backward pass; the key-padding bias is optional.
@@ -13,7 +13,7 @@
 //   act_bwd_kernel, colsum_kernel      GELU / tanh / ReLU backward, bias gradient
 //   dropout_bf16_kernel                hash dropout (same kernel re-applies the mask in backward)
 //   embed3_fwd_kernel / embed3_bwd_kernel   word + position + token-type embedding gather / scatter-add
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace slb {
 
@@ -30,7 +30,6 @@ __device__ __forceinline__ float drop_scale(uint32_t seed, uint32_t idx, float p
 __device__ __forceinline__ uint32_t mix_seed(uint32_t seed, const uint32_t* ofs) {
   return ofs ? seed + __ldg(ofs) * 0x9E3779B9u : seed;
 }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // byte offset of the 16-byte chunk holding columns [c8*8, c8*8+8) of row r inside a [128 rows][128 cols] bf16 tile
 // stored as two 64-column panels of 128-byte rows with the 128B swizzle (what TMA writes for a {64, 128} box).
@@ -56,35 +55,48 @@ struct AttnParams {
 };
 
 static constexpr int ATT_TILE = 16384;                       // one [128][64] bf16 box
-static constexpr int ATT_FWD_SMEM = 3 * ATT_TILE + 1024 + 1024;   // P re-uses the Q/K tiles -> 4 CTAs per SM
+static constexpr int ATT_FWD_SMEM = 5 * ATT_TILE + 1024 + 1024;   // Q, K, V, P -> 2 CTAs per SM
 static constexpr int ATT_BWD_SMEM = 4 * ATT_TILE + 2 * 32768 + 1024 + 1024;
 
-// store `n` fp32 accumulator columns (a 32-wide TMEM chunk) as bf16, 16-byte vectors
-__device__ __forceinline__ void store_bf16x32(__nv_bfloat16* dst, const uint32_t (&v)[32], float mul) {
-  uint4* o4 = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    o4[j] = make_uint4(pack_bf16x2(__uint_as_float(v[8 * j]) * mul, __uint_as_float(v[8 * j + 1]) * mul),
-                       pack_bf16x2(__uint_as_float(v[8 * j + 2]) * mul, __uint_as_float(v[8 * j + 3]) * mul),
-                       pack_bf16x2(__uint_as_float(v[8 * j + 4]) * mul, __uint_as_float(v[8 * j + 5]) * mul),
-                       pack_bf16x2(__uint_as_float(v[8 * j + 6]) * mul, __uint_as_float(v[8 * j + 7]) * mul));
+// Rows of a thread inside a warpgroup's 64-row wgmma fragment: r and r + 8 (plus 64 for the second half of the tile);
+// element d[4i + e] sits in column 8i + 2 * (lane % 4) + (e & 1).
+__device__ __forceinline__ int frag_row(int half) { return 64 * half + 16 * (threadIdx.x >> 5) + (lane_id() >> 2); }
+__device__ __forceinline__ int frag_col(int i) { return 8 * i + 2 * (lane_id() & 3); }
+// sum / max over the four threads that share a row of the fragment
+__device__ __forceinline__ float quad_sum(float x) {
+  x += __shfl_xor_sync(0xffffffffu, x, 1);
+  return x + __shfl_xor_sync(0xffffffffu, x, 2);
+}
+__device__ __forceinline__ float quad_max(float x) {
+  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+}
+// two adjacent bf16 values at (row, col) of a [128][128] tile in the two-panel 128B-swizzled layout (col even)
+__device__ __forceinline__ void st_tile_pair(uint8_t* tile, int row, int col, float lo, float hi) {
+  *reinterpret_cast<uint32_t*>(tile + sw128_chunk(row, col >> 3) + (col & 7) * 2) = pack_bf16x2(lo, hi);
 }
 
-// Write one head's slice of a [128][64] accumulator at TMEM column `tcol`: columns [n_off, n_off + Dh) of the tile.
-__device__ __forceinline__ void store_head_tile(uint32_t tmem_lane_base, int tcol, __nv_bfloat16* dst_row, int n_off,
-                                                int Dh, bool row_ok, float mul) {
-#pragma unroll 1
-  for (int c = 0; c < 64; c += 32) {
-    if (c < n_off || c >= n_off + Dh) continue;                // warp-uniform
-    uint32_t v[32];
-    tmem_ld32(tmem_lane_base + tcol + c, v);
-    tmem_ld_wait();
-    if (row_ok) store_bf16x32(dst_row + (c - n_off), v, mul);
+// Write one head's slice of a 64 x 64 accumulator fragment (rows [64 * half, 64 * half + 64) of the tile): columns
+// [n_off, n_off + Dh) go to dst[row * ld + col - n_off] for rows < S, scaled by mul[0] / mul[1] (rows r / r + 8).
+__device__ __forceinline__ void store_head_frag(const float (&o)[32], int half, __nv_bfloat16* dst, long long ld, int n_off,
+                                                int Dh, int S, const float (&mul)[2]) {
+  const int r = frag_row(half);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int col = frag_col(i);
+    if (col < n_off || col >= n_off + Dh) continue;
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = r + 8 * hh;
+      if (row < S)
+        *reinterpret_cast<uint32_t*>(dst + row * ld + col - n_off) =
+            pack_bf16x2(o[4 * i + 2 * hh] * mul[hh], o[4 * i + 2 * hh + 1] * mul[hh]);
+    }
   }
 }
 
 // ----------------------------------------------------------------------------- attention forward
-__global__ void __launch_bounds__(128, 4)
+__global__ void __launch_bounds__(128, 2)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -92,117 +104,102 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   uint8_t* sQ = smem;
   uint8_t* sK = smem + ATT_TILE;
   uint8_t* sV = smem + 2 * ATT_TILE;
-  uint8_t* sP = smem;                  // [128][128] bf16, two panels: overwrites Q and K once S = Q K^T has retired
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 3 * ATT_TILE);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
+  uint8_t* sP = smem + 3 * ATT_TILE;   // [128][128] bf16, two panels
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 5 * ATT_TILE);
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int b = blockIdx.x / p.H, h = blockIdx.x - b * p.H;
   const int qc = p.q_col + h * p.Dh, kc = p.k_col + h * p.Dh, vc = p.v_col + h * p.Dh;
   const int ksteps = p.Dh >> 4;
 
   if (tid == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-    for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+    mbar_init(&bars[0], 1);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc<128>(tmem_slot);       // S [0,128); O re-uses [0,64) after the softmax has consumed S
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-
   if (tid == 0) {
     mbar_expect_tx(&bars[0], 3 * ATT_TILE);
     tma_load_2d(sQ, &tmQ, &bars[0], qc & ~63, b * p.S);
     tma_load_2d(sK, &tmK, &bars[0], kc & ~63, b * p.S);
     tma_load_2d(sV, &tmV, &bars[0], vc & ~63, b * p.S);
-    mbar_wait(&bars[0], 0);
-    tc_fence_after();
-    const uint32_t idesc = umma_idesc_bf16(128, 128, false, false);
-    const uint32_t qa = smem_u32(sQ) + ((qc & 63) >> 4) * 32, ka = smem_u32(sK) + ((kc & 63) >> 4) * 32;
-    for (int k = 0; k < ksteps; ++k)                                     // S = Q K^T  -> TMEM [0, 128)
-      umma_bf16(tmem, umma_desc_sw128(qa + k * 32, 16, 1024), umma_desc_sw128(ka + k * 32, 16, 1024), idesc, k != 0);
-    umma_commit(&bars[1]);
   }
-  __syncwarp();
-  mbar_wait(&bars[1], 0);
-  tc_fence_after();
+  mbar_wait(&bars[0], 0);
 
-  // ---- softmax: thread = query row, two passes over the TMEM row
-  const int row = tid;
-  const uint32_t lane_base = tmem + (static_cast<uint32_t>(warp * 32) << 16);
+  const uint32_t qa = smem_u32(sQ) + ((qc & 63) >> 4) * 32, ka = smem_u32(sK) + ((kc & 63) >> 4) * 32;
   const float* kb = p.key_bias ? p.key_bias + static_cast<long long>(b) * p.S : nullptr;
   constexpr float LOG2E = 1.4426950408889634f;
-  float mx = -INFINITY;
-#pragma unroll 1
-  for (int c = 0; c < 128; c += 32) {
-    if (c >= p.S) break;
-    uint32_t v[32];
-    tmem_ld32(lane_base + c, v);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const int col = c + j;
-      if (col < p.S) mx = fmaxf(mx, __uint_as_float(v[j]) * p.scale + (kb ? __ldg(kb + col) : 0.f));
-    }
-  }
-  float sum = 0.f;
   const uint32_t seed = mix_seed(p.seed, p.seed_ofs);
   const float inv_keep = p.p_drop > 0.f ? 1.f / (1.f - p.p_drop) : 1.f;
-  const uint32_t idx0 = (static_cast<uint32_t>(blockIdx.x) * 128u + row) * 128u;
+  float inv_sum[2][2];
+  // ---- S = Q K^T and the softmax, one 64-row half of the tile at a time (fragment rows r, r + 8)
 #pragma unroll 1
-  for (int c = 0; c < 128; c += 32) {
-    float e[32];
-    if (c < p.S) {
-      uint32_t v[32];
-      tmem_ld32(lane_base + c, v);
-      tmem_ld_wait();
+  for (int half = 0; half < 2; ++half) {
+    float s[64];
+    wgmma_fence();
+    for (int k = 0; k < ksteps; ++k)
+      wgmma_bf16_n128<0, 0>(s, wg_desc_sw128(qa + half * 8192 + k * 32, 16, 1024), wg_desc_sw128(ka + k * 32, 16, 1024), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    const int r = frag_row(half);
+    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int col = c + j;
-        float x = 0.f;
-        if (col < p.S) {
-          x = exp2f((__uint_as_float(v[j]) * p.scale + (kb ? __ldg(kb + col) : 0.f) - mx) * LOG2E);
-          sum += x;
-          if (p.p_drop > 0.f) x *= drop_scale(seed, idx0 + col, p.p_drop, inv_keep);
-        }
-        e[j] = x;
+    for (int i = 0; i < 16; ++i) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int col = frag_col(i) + (e & 1);
+        const float x = col < p.S ? s[4 * i + e] * p.scale + (kb ? __ldg(kb + col) : 0.f) : -INFINITY;
+        s[4 * i + e] = x;
+        mx[e >> 1] = fmaxf(mx[e >> 1], x);
       }
-    } else {
+    }
+    mx[0] = quad_max(mx[0]);
+    mx[1] = quad_max(mx[1]);
+    float sum[2] = {0.f, 0.f};
 #pragma unroll
-      for (int j = 0; j < 32; ++j) e[j] = 0.f;
+    for (int i = 0; i < 16; ++i) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = r + 8 * hh;
+        const uint32_t idx0 = (static_cast<uint32_t>(blockIdx.x) * 128u + row) * 128u;
+        float e2[2];
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+          const int col = frag_col(i) + t;
+          float x = 0.f;
+          if (col < p.S) {
+            x = exp2f((s[4 * i + 2 * hh + t] - mx[hh]) * LOG2E);
+            sum[hh] += x;
+            if (p.p_drop > 0.f) x *= drop_scale(seed, idx0 + col, p.p_drop, inv_keep);
+          }
+          e2[t] = x;
+        }
+        st_tile_pair(sP, row, frag_col(i), e2[0], e2[1]);
+      }
     }
 #pragma unroll
-    for (int j = 0; j < 4; ++j)
-      *reinterpret_cast<uint4*>(sP + sw128_chunk(row, (c >> 3) + j)) =
-          make_uint4(pack_bf16x2(e[8 * j], e[8 * j + 1]), pack_bf16x2(e[8 * j + 2], e[8 * j + 3]),
-                     pack_bf16x2(e[8 * j + 4], e[8 * j + 5]), pack_bf16x2(e[8 * j + 6], e[8 * j + 7]));
+    for (int hh = 0; hh < 2; ++hh) {
+      sum[hh] = quad_sum(sum[hh]);
+      inv_sum[half][hh] = 1.f / sum[hh];
+      const int row = r + 8 * hh;
+      if (row < p.S && (lane_id() & 3) == 0) p.lse[static_cast<long long>(blockIdx.x) * 128 + row] = mx[hh] + logf(sum[hh]);
+    }
   }
   fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core (async proxy)
-  tc_fence_before();
   __syncthreads();
-  if (tid == 0) {
-    tc_fence_after();
-    const uint32_t idesc = umma_idesc_bf16(128, 64, false, true);       // A = P (K-major), B = V (MN-major)
-    const uint32_t pa = smem_u32(sP), va = smem_u32(sV);
-    for (int k = 0; k < 8; ++k)                                          // O~ = P~ V  -> TMEM [0, 64)
-      umma_bf16(tmem, umma_desc_sw128(pa + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
-                umma_desc_sw128(va + k * 2048, 16384, 1024), idesc, k != 0);
-    umma_commit(&bars[2]);
-  }
-  __syncwarp();
-  mbar_wait(&bars[2], 0);
-  tc_fence_after();
-  const bool row_ok = row < p.S;
-  const long long grow = static_cast<long long>(b) * p.S + row;
-  store_head_tile(lane_base, 0, p.out + grow * p.ldo + h * p.Dh, vc & 63, p.Dh, row_ok, 1.f / sum);
-  if (row_ok) p.lse[static_cast<long long>(blockIdx.x) * 128 + row] = mx + logf(sum);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<128>(tmem);
+  // ---- O~ = P~ V  (A = P K-major, B = V MN-major), normalised by the row sums on the way out
+  const uint32_t pa = smem_u32(sP), va = smem_u32(sV);
+  __nv_bfloat16* dst = p.out + static_cast<long long>(b) * p.S * p.ldo + h * p.Dh;
+#pragma unroll 1
+  for (int half = 0; half < 2; ++half) {
+    float o[32];
+    wgmma_fence();
+    for (int k = 0; k < 8; ++k)
+      wgmma_bf16_n64<0, 1>(o, wg_desc_sw128(pa + half * 8192 + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
+                           wg_desc_sw128(va + k * 2048, 16384, 1024), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    store_head_frag(o, half, dst, p.ldo, vc & 63, p.Dh, p.S, inv_sum[half]);
   }
 }
 
@@ -220,153 +217,115 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   uint8_t* sP = smem + 4 * ATT_TILE;                 // dropped probabilities  P~ = P * keep/(1-p)
   uint8_t* sdS = sP + 32768;                          // dS = P * (dP~ - D) * scale
   uint64_t* bars = reinterpret_cast<uint64_t*>(sdS + 32768);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int b = blockIdx.x / p.H, h = blockIdx.x - b * p.H;
   const int qc = p.q_col + h * p.Dh, kc = p.k_col + h * p.Dh, vc = p.v_col + h * p.Dh, oc = p.do_col + h * p.Dh;
   const int ksteps = p.Dh >> 4;
 
   if (tid == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
-    for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+    mbar_init(&bars[0], 1);
     mbar_fence_init();
   }
-  if (warp == 0) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  // TMEM columns: S [0,128)  dP [128,256)  dV [256,320)  dQ [320,384)  dK [384,448)
-
   if (tid == 0) {
     mbar_expect_tx(&bars[0], 4 * ATT_TILE);
     tma_load_2d(sQ, &tmQ, &bars[0], qc & ~63, b * p.S);
     tma_load_2d(sK, &tmK, &bars[0], kc & ~63, b * p.S);
     tma_load_2d(sV, &tmV, &bars[0], vc & ~63, b * p.S);
     tma_load_2d(sdO, &tmDO, &bars[0], oc & ~63, b * p.S);
-    mbar_wait(&bars[0], 0);
-    tc_fence_after();
-    const uint32_t idesc = umma_idesc_bf16(128, 128, false, false);
-    const uint32_t qa = smem_u32(sQ) + ((qc & 63) >> 4) * 32, ka = smem_u32(sK) + ((kc & 63) >> 4) * 32;
-    const uint32_t va = smem_u32(sV) + ((vc & 63) >> 4) * 32, oa = smem_u32(sdO) + ((oc & 63) >> 4) * 32;
-    for (int k = 0; k < ksteps; ++k)                                     // S = Q K^T
-      umma_bf16(tmem, umma_desc_sw128(qa + k * 32, 16, 1024), umma_desc_sw128(ka + k * 32, 16, 1024), idesc, k != 0);
-    for (int k = 0; k < ksteps; ++k)                                     // dP = dO V^T
-      umma_bf16(tmem + 128, umma_desc_sw128(oa + k * 32, 16, 1024), umma_desc_sw128(va + k * 32, 16, 1024), idesc,
-                k != 0);
-    umma_commit(&bars[1]);
   }
-  __syncwarp();
-  mbar_wait(&bars[1], 0);
-  tc_fence_after();
+  mbar_wait(&bars[0], 0);
 
-  const int row = tid;
-  const bool row_ok = row < p.S;
-  const uint32_t lane_base = tmem + (static_cast<uint32_t>(warp * 32) << 16);
   const float* kb = p.key_bias ? p.key_bias + static_cast<long long>(b) * p.S : nullptr;
   constexpr float LOG2E = 1.4426950408889634f;
-  const float lse = row_ok ? p.lse[static_cast<long long>(blockIdx.x) * 128 + row] : 0.f;
   const uint32_t seed = mix_seed(p.seed, p.seed_ofs);
   const float inv_keep = p.p_drop > 0.f ? 1.f / (1.f - p.p_drop) : 1.f;
-  const uint32_t idx0 = (static_cast<uint32_t>(blockIdx.x) * 128u + row) * 128u;
-
-  // pass 1: P~ -> smem, D = rowsum(P~ * dP); the probabilities (bf16) and the dropout mask stay in registers
-  float D = 0.f;
-  uint32_t pk[64], mbits[4];
+  {
+    const uint32_t qa = smem_u32(sQ) + ((qc & 63) >> 4) * 32, ka = smem_u32(sK) + ((kc & 63) >> 4) * 32;
+    const uint32_t va = smem_u32(sV) + ((vc & 63) >> 4) * 32, oa = smem_u32(sdO) + ((oc & 63) >> 4) * 32;
+#pragma unroll 1
+    for (int half = 0; half < 2; ++half) {
+      float s[64], g[64];
+      wgmma_fence();
+      for (int k = 0; k < ksteps; ++k)                                   // S = Q K^T
+        wgmma_bf16_n128<0, 0>(s, wg_desc_sw128(qa + half * 8192 + k * 32, 16, 1024), wg_desc_sw128(ka + k * 32, 16, 1024), k != 0);
+      for (int k = 0; k < ksteps; ++k)                                   // dP = dO V^T
+        wgmma_bf16_n128<0, 0>(g, wg_desc_sw128(oa + half * 8192 + k * 32, 16, 1024), wg_desc_sw128(va + k * 32, 16, 1024), k != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      const int r = frag_row(half);
+      float lse[2], D[2] = {0.f, 0.f};
 #pragma unroll
-  for (int ci = 0; ci < 4; ++ci) {
-    const int c = ci * 32;
-    float e[32], pr[32];
-    uint32_t mb = 0;
-    if (c < p.S) {                        // warp-uniform: tcgen05.ld is .sync.aligned, row_ok only predicates the math
-      uint32_t s[32], g[32];
-      tmem_ld32(lane_base + c, s);
-      tmem_ld32(lane_base + 128 + c, g);
-      tmem_ld_wait();
+      for (int hh = 0; hh < 2; ++hh)
+        lse[hh] = (r + 8 * hh) < p.S ? p.lse[static_cast<long long>(blockIdx.x) * 128 + r + 8 * hh] : 0.f;
+      // P -> s, dP * mask -> g, P~ -> smem, D = rowsum(P~ * dP)
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int col = c + j;
-        float x = 0.f, mk = 1.f;
-        if (col < p.S && row_ok) {
-          x = exp2f((__uint_as_float(s[j]) * p.scale + (kb ? __ldg(kb + col) : 0.f) - lse) * LOG2E);
-          if (p.p_drop > 0.f) mk = drop_scale(seed, idx0 + col, p.p_drop, inv_keep);
+      for (int i = 0; i < 16; ++i) {
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row = r + 8 * hh;
+          const uint32_t idx0 = (static_cast<uint32_t>(blockIdx.x) * 128u + row) * 128u;
+          float e2[2];
+#pragma unroll
+          for (int t = 0; t < 2; ++t) {
+            const int col = frag_col(i) + t, j = 4 * i + 2 * hh + t;
+            float x = 0.f, mk = 1.f;
+            if (col < p.S && row < p.S) {
+              x = exp2f((s[j] * p.scale + (kb ? __ldg(kb + col) : 0.f) - lse[hh]) * LOG2E);
+              if (p.p_drop > 0.f) mk = drop_scale(seed, idx0 + col, p.p_drop, inv_keep);
+            }
+            s[j] = x;
+            g[j] *= mk;
+            D[hh] += x * g[j];
+            e2[t] = x * mk;
+          }
+          st_tile_pair(sP, row, frag_col(i), e2[0], e2[1]);
         }
-        pr[j] = x;
-        if (mk != 0.f) mb |= 1u << j;
-        x *= mk;
-        D += x * __uint_as_float(g[j]);
-        e[j] = x;
       }
-    } else {
+      D[0] = quad_sum(D[0]);
+      D[1] = quad_sum(D[1]);
+      // dS = P * (dP * mask - D) * scale -> smem
 #pragma unroll
-      for (int j = 0; j < 32; ++j) { e[j] = 0.f; pr[j] = 0.f; }
-    }
-    mbits[ci] = mb;
+      for (int i = 0; i < 16; ++i) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) pk[ci * 16 + j] = pack_bf16x2(pr[2 * j], pr[2 * j + 1]);
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      *reinterpret_cast<uint4*>(sP + sw128_chunk(row, (c >> 3) + j)) =
-          make_uint4(pack_bf16x2(e[8 * j], e[8 * j + 1]), pack_bf16x2(e[8 * j + 2], e[8 * j + 3]),
-                     pack_bf16x2(e[8 * j + 4], e[8 * j + 5]), pack_bf16x2(e[8 * j + 6], e[8 * j + 7]));
-  }
-  // pass 2: dS = P * (dP * mask - D) * scale -> smem   (no second exp / hash: P and the mask come from registers)
-#pragma unroll
-  for (int ci = 0; ci < 4; ++ci) {
-    const int c = ci * 32;
-    float e[32];
-    if (c < p.S) {
-      uint32_t g[32];
-      tmem_ld32(lane_base + 128 + c, g);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const __nv_bfloat162 h2 = *reinterpret_cast<const __nv_bfloat162*>(&pk[ci * 16 + (j >> 1)]);
-        const float prj = __bfloat162float((j & 1) ? h2.y : h2.x);
-        const float mk = ((mbits[ci] >> j) & 1u) ? inv_keep : 0.f;
-        e[j] = prj * (__uint_as_float(g[j]) * mk - D) * p.scale;
+        for (int hh = 0; hh < 2; ++hh) {
+          const int j = 4 * i + 2 * hh;
+          st_tile_pair(sdS, r + 8 * hh, frag_col(i), s[j] * (g[j] - D[hh]) * p.scale, s[j + 1] * (g[j + 1] - D[hh]) * p.scale);
+        }
       }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) e[j] = 0.f;
     }
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      *reinterpret_cast<uint4*>(sdS + sw128_chunk(row, (c >> 3) + j)) =
-          make_uint4(pack_bf16x2(e[8 * j], e[8 * j + 1]), pack_bf16x2(e[8 * j + 2], e[8 * j + 3]),
-                     pack_bf16x2(e[8 * j + 4], e[8 * j + 5]), pack_bf16x2(e[8 * j + 6], e[8 * j + 7]));
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  if (tid == 0) {
-    tc_fence_after();
-    const uint32_t pa = smem_u32(sP), sa = smem_u32(sdS), qa = smem_u32(sQ), ka = smem_u32(sK), oa = smem_u32(sdO);
-    const uint32_t i_tt = umma_idesc_bf16(128, 64, true, true), i_nt = umma_idesc_bf16(128, 64, false, true);
+  const uint32_t pa = smem_u32(sP), sa = smem_u32(sdS), qa = smem_u32(sQ), ka = smem_u32(sK), oa = smem_u32(sdO);
+  const long long row0 = static_cast<long long>(b) * p.S;
+  const float one[2] = {1.f, 1.f};
+#pragma unroll 1
+  for (int half = 0; half < 2; ++half) {
+    float o[32];
+    wgmma_fence();
     for (int k = 0; k < 8; ++k)        // dV[key][d] = sum_q P~[q][key] dO[q][d]   (A = P~ MN-major, B = dO MN-major)
-      umma_bf16(tmem + 256, umma_desc_sw128(pa + k * 2048, 16384, 1024), umma_desc_sw128(oa + k * 2048, 16384, 1024),
-                i_tt, k != 0);
+      wgmma_bf16_n64<1, 1>(o, wg_desc_sw128(pa + half * 16384 + k * 2048, 16384, 1024), wg_desc_sw128(oa + k * 2048, 16384, 1024),
+                           k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    store_head_frag(o, half, p.dv + row0 * p.lddv + p.dv_col + h * p.Dh, p.lddv, oc & 63, p.Dh, p.S, one);
+    wgmma_fence();
     for (int k = 0; k < 8; ++k)        // dQ[q][d] = sum_key dS[q][key] K[key][d]  (A = dS K-major, B = K MN-major)
-      umma_bf16(tmem + 320, umma_desc_sw128(sa + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
-                umma_desc_sw128(ka + k * 2048, 16384, 1024), i_nt, k != 0);
+      wgmma_bf16_n64<0, 1>(o, wg_desc_sw128(sa + half * 8192 + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
+                           wg_desc_sw128(ka + k * 2048, 16384, 1024), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    store_head_frag(o, half, p.dq + row0 * p.lddq + p.dq_col + h * p.Dh, p.lddq, kc & 63, p.Dh, p.S, one);
+    wgmma_fence();
     for (int k = 0; k < 8; ++k)        // dK[key][d] = sum_q dS[q][key] Q[q][d]    (A = dS MN-major, B = Q MN-major)
-      umma_bf16(tmem + 384, umma_desc_sw128(sa + k * 2048, 16384, 1024), umma_desc_sw128(qa + k * 2048, 16384, 1024),
-                i_tt, k != 0);
-    umma_commit(&bars[2]);
-  }
-  __syncwarp();
-  mbar_wait(&bars[2], 0);
-  tc_fence_after();
-  const long long grow = static_cast<long long>(b) * p.S + row;
-  store_head_tile(lane_base, 256, p.dv + grow * p.lddv + p.dv_col + h * p.Dh, oc & 63, p.Dh, row_ok, 1.f);
-  store_head_tile(lane_base, 320, p.dq + grow * p.lddq + p.dq_col + h * p.Dh, kc & 63, p.Dh, row_ok, 1.f);
-  store_head_tile(lane_base, 384, p.dk + grow * p.lddk + p.dk_col + h * p.Dh, qc & 63, p.Dh, row_ok, 1.f);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem);
+      wgmma_bf16_n64<1, 1>(o, wg_desc_sw128(sa + half * 16384 + k * 2048, 16384, 1024), wg_desc_sw128(qa + k * 2048, 16384, 1024),
+                           k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    store_head_frag(o, half, p.dk + row0 * p.lddk + p.dk_col + h * p.Dh, p.lddk, qc & 63, p.Dh, p.S, one);
   }
 }
 
@@ -718,7 +677,7 @@ int slb_act_bwd(const void* dy, const void* ref, void* dz, long long n, int kind
   if (n & 1) return -3;
   const long long n2 = n / 2;
   int grid = static_cast<int>((n2 + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   act_bwd_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(dy),
                                        reinterpret_cast<const __nv_bfloat16*>(ref),
                                        reinterpret_cast<__nv_bfloat16*>(dz), n2, kind);
@@ -735,7 +694,7 @@ int slb_dropout_bf16(const void* x, void* y, long long n, float p, unsigned seed
   if (n & 1 || n >= (1ll << 32)) return -3;
   const long long n2 = n / 2;
   int grid = static_cast<int>((n2 + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   dropout_bf16_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x),
                                             reinterpret_cast<__nv_bfloat16*>(y), n2, p, seed, seed_ofs);
   return check_launch();

@@ -1,4 +1,4 @@
-// One warp-specialised tcgen05 GEMM pipeline, instantiated for every GEMM-shaped op of the
+// One warp-specialised wgmma GEMM pipeline, instantiated for every GEMM-shaped op of the
 // split-learning stages (SURVEY §2.7 G1-G3, G6):
 //
 //   MODE_CONV   conv3x3 s1 p1 forward and input-gradient as implicit GEMM.
@@ -10,15 +10,16 @@
 //   MODE_GEMM   plain C[M,N] (+)= A * B with any major combination: the three Linear GEMMs
 //               (swap-AB so the 4096-wide dimension sits on the MMA M axis).
 //
-// Roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM alloc + single-thread MMA issue,
-// warps 2..5 = epilogue (TMEM lane quarter = warp_idx % 4).  BLOCK_M = 128 (UMMA M),
-// BLOCK_K = one 128-byte swizzle row, fp32 accumulators in TMEM.
+// Roles (288 threads): warps 0..7 = two consumer warpgroups issuing wgmma (rows [0,64) and [64,128)
+// of the tile, fp32 accumulators in registers), warp 8 = TMA producer.  BLOCK_M = 128, BLOCK_K = one
+// 128-byte swizzle row.  After the mainloop the accumulators go to shared memory and warps 0..3 run the
+// epilogue with one output row per thread.
 //
 // Two operand precisions share the pipeline (template parameter T, sm100.cuh OperandTraits):
-//   float          fp32 tensors in HBM and shared memory, tcgen05.mma kind::tf32 (the reference's precision: PyTorch
+//   float          fp32 tensors in HBM and shared memory, wgmma tf32 (the reference's precision: PyTorch
 //                  runs cuDNN convolutions on TF32 tensor cores by default, SURVEY §2.7 note), BLOCK_K = 32, fp32 outputs
-//   __nv_bfloat16  bf16 operands / outputs, kind::f16, BLOCK_K = 64 (opt-in fast mode)
-#include "sm100.cuh"
+//   __nv_bfloat16  bf16 operands / outputs, wgmma bf16, BLOCK_K = 64 (opt-in fast mode)
+#include "sm90.cuh"
 
 namespace slb {
 
@@ -27,7 +28,7 @@ enum { EPI_BF16 = 0 /* activation-typed store (bf16 or fp32) */, EPI_F32_ATOMIC 
 
 struct GemmParams {
   // generic
-  int M, N;             // logical output extent (rows on TMEM lanes, cols on TMEM columns)
+  int M, N;             // logical output extent (rows x columns of the accumulator tiles)
   int k_iters;          // total K iterations of 64
   int k_split;          // gridDim.z
   int a_mn, b_mn;       // operand majors (1 = MN-major)
@@ -74,6 +75,7 @@ struct GemmParams {
   int act;                        // 0 none, 1 ReLU, 2 GELU (erf), 3 tanh
   __nv_bfloat16* aux_out;         // [M][ldo] or nullptr
   const __nv_bfloat16* residual;  // [M][ldo] or nullptr
+  Det det;                        // reproducible reductions: BN statistics across m-tiles, split-K turns without tile_counters
 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {
@@ -83,15 +85,21 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   return x;
 }
 
-template <int BLOCK_N>
+template <int BLOCK_N, typename T>
 struct SmemLayout {
   static constexpr int A_BYTES = 128 * 128;      // 16 KB
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BLOCK_N >= 256) ? 4 : (BLOCK_N >= 128 ? 5 : 6);
-  static constexpr int TILE_BYTES = STAGES * STAGE_BYTES;
+  static constexpr int STAGING = OperandTraits<T>::TF32 ? STAGE_BYTES : 0;   // K-major copies of MN-major fp32 operands
+  static constexpr int STAGES_FIT = (196 * 1024 - STAGING) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT < 6 ? STAGES_FIT : 6;
+  static constexpr int TILE_BYTES = STAGES * STAGE_BYTES + STAGING;
+  // once the MMAs are done the ring holds the epilogue's transpose tiles [0, 17 KB) and the fp32 accumulator tile
+  static constexpr int ACC_OFF = 17 * 1024;
+  static constexpr int ACC_LD = BLOCK_N + 4;     // row pitch in floats: 16-byte row reads without bank conflicts
   static constexpr int BAR_BYTES = 4096;
   static constexpr int TOTAL = TILE_BYTES + BAR_BYTES + 1024 /*align slack*/;
+  static_assert(ACC_OFF + 128 * ACC_LD * 4 <= TILE_BYTES, "accumulator tile must fit in the pipeline buffers");
 };
 
 // Sum of v[c] over the 32 lanes of a warp for every c in 0..31; lane j returns column j.
@@ -217,24 +225,23 @@ __device__ __forceinline__ void stat_terms(const GemmParams& p, int row, bool ro
 // BNB: instantiate the upstream-BatchNorm-backward epilogue (dgrad only).  A separate instantiation on purpose: with the
 // code in the common kernel every conv paid ~1.8 % (205 vs 154 registers; same-box A/B, profiles/README.md).
 template <int MODE, int BLOCK_N, typename T, bool BNB = false>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(288, 1)
 umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
-  using L = SmemLayout<BLOCK_N>;
+  using L = SmemLayout<BLOCK_N, T>;
   using OT = OperandTraits<T>;
   constexpr int KE = OT::KE;                       // K elements per stage == elements per MN-major group (128 bytes)
   constexpr int GROUP_BYTES = KE * 128;            // one MN-major group: KE k-rows of 128 bytes
   static_assert(!BNB || !OT::TF32, "the fused BatchNorm-backward epilogue is a bf16-only option");
-  constexpr int TMEM_COLS = BLOCK_N < 32 ? 32 : BLOCK_N;
   pdl_trigger();                      // the next kernel may start its prologue now
   // __align__(1024): the dynamic shared-memory window starts on a swizzle-atom boundary, and — unlike rounding the pointer
   // up by hand through an integer cast — the compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::TILE_BYTES);
   uint64_t* empty_bar = full_bar + L::STAGES;
-  uint64_t* accum_bar = empty_bar + L::STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
-  float* s_stats = reinterpret_cast<float*>(tmem_slot + 4);   // [2][BLOCK_N] floats (<= 2 KB of the 4 KB tail)
+  uint32_t* s_flag = reinterpret_cast<uint32_t*>(empty_bar + L::STAGES);
+  float* s_stats = reinterpret_cast<float*>(s_flag + 4);      // [2][BLOCK_N] floats (<= 2 KB of the 4 KB tail)
+  float* s_acc = reinterpret_cast<float*>(smem + L::ACC_OFF); // [128][ACC_LD] accumulators for the epilogue
 
   const int warp = threadIdx.x >> 5;
   const int m_tile = blockIdx.x, n_tile = blockIdx.y, z = blockIdx.z;
@@ -254,23 +261,18 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < L::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);                 // one arrival per consumer warpgroup
     }
-    mbar_init(accum_bar, 1);
     mbar_fence_init();
+    s_flag[1] = 0;
   }
-  if (threadIdx.x == 32) tmem_slot[1] = 0;
-  if (warp == 1) tmem_alloc<TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   if (threadIdx.x == 0) SLB_STAMP(1);
   pdl_wait();                         // predecessor grids complete + visible; prologue above overlapped with their tail
   if (threadIdx.x == 0) SLB_STAMP(2);
 
   if (my_iters > 0) {
-    if (warp == 0) {
+    if (warp == 8) {
       // ============================== TMA producer ==============================
       if (elect_one()) {
         int stage = 0;
@@ -341,49 +343,32 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
         }
       }
-    } else if (warp == 1) {
-      // ============================== MMA issuer ==============================
-      const uint32_t idesc = umma_idesc(128, BLOCK_N, p.a_mn != 0, p.b_mn != 0, OT::FMT);
+    } else {
+      // ========================= two wgmma warpgroups, then the epilogue (warps 0..3) =========================
+      const int et = threadIdx.x;                  // 0..127: epilogue thread id
+      const bool want_stats = (p.col_sum != nullptr);
+      // the bias of this tile's columns is staged in shared memory before the mainloop (32 dependent-latency global
+      // loads per 32-column chunk would otherwise sit on the epilogue's critical path)
+      float* s_bias = s_stats + 2 * BLOCK_N;
+      if (warp < 4) {
+        for (int i = et; i < 2 * BLOCK_N; i += 128) s_stats[i] = 0.f;
+        for (int i = et; i < BLOCK_N; i += 128) s_bias[i] = (p.bias != nullptr && n0 + i < p.N) ? __ldg(p.bias + n0 + i) : 0.f;
+      }
+      float acc[BLOCK_N / 2];
       int stage = 0;
       uint32_t phase = 0;
-      for (int it = 0; it < my_iters; ++it) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (it == 0 && lane_id() == 0) SLB_STAMP(4);          // first operands have landed
-        if (it == my_iters - 1 && lane_id() == 0) SLB_STAMP(5);  // last operands have landed
-        if (elect_one()) {
-          const uint32_t a_base = smem_u32(smem + stage * L::STAGE_BYTES);
-          const uint32_t b_base = a_base + L::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t da = p.a_mn ? umma_desc_mn<T>(a_base, k, GROUP_BYTES) : umma_desc_sw128(a_base + k * 32, 16, 1024);
-            const uint64_t db = p.b_mn ? umma_desc_mn<T>(b_base, k, GROUP_BYTES) : umma_desc_sw128(b_base + k * 32, 16, 1024);
-            umma_issue<T>(tmem_base, da, db, idesc, (it | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);                  // frees this smem stage once the MMAs retire
-          if (it == my_iters - 1) umma_commit(accum_bar);  // accumulator complete
-        }
-        __syncwarp();
-        if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
-      }
-    } else {
-      // ============================== epilogue ==============================
-      const int q = warp & 3;                       // TMEM lane quarter owned by this warp
-      const int row = m0 + q * 32 + lane_id();      // output row of this thread
-      const int et = (warp - 2) * 32 + lane_id();   // 0..127 epilogue thread id
-      const bool want_stats = (p.col_sum != nullptr);
-      // the bias of this tile's columns is staged in shared memory while the mainloop runs (32 dependent-latency global
-      // loads per 32-column chunk used to sit on the epilogue's critical path: 1.3 us per chunk)
-      float* s_bias = s_stats + 2 * BLOCK_N;
-      for (int i = et; i < 2 * BLOCK_N; i += 128) s_stats[i] = 0.f;
-      for (int i = et; i < BLOCK_N; i += 128) s_bias[i] = (p.bias != nullptr && n0 + i < p.N) ? __ldg(p.bias + n0 + i) : 0.f;
-      asm volatile("bar.sync 1, 128;");
-      // warp-private transpose tile for the statistics: the pipeline buffers are free once the accumulator is complete
-      float* s_tr = reinterpret_cast<float*>(smem) + (warp - 2) * (32 * 33);
-      static_assert(L::TILE_BYTES >= 4 * 32 * 33 * 4, "transpose tiles must fit in the pipeline buffers");
-      mbar_wait(accum_bar, 0);
-      tc_fence_after();
+      wg_mainloop<T, BLOCK_N>(smem, smem + L::STAGES * L::STAGE_BYTES, L::STAGE_BYTES, L::A_BYTES, L::STAGES, full_bar,
+                              empty_bar, my_iters, p.a_mn, p.b_mn, acc, stage, phase);
       if (et == 0) SLB_STAMP(6);                               // accumulator complete
+      asm volatile("bar.sync 2, 256;" ::: "memory");           // no MMA reads the ring any more
+      wg_store_acc<BLOCK_N>(s_acc + (threadIdx.x >> 7) * 64 * L::ACC_LD, L::ACC_LD, acc);
+      asm volatile("bar.sync 2, 256;" ::: "memory");
+      if (warp < 4) {
+      const int q = warp;                           // rows [32q, 32q + 32) of the tile
+      const int row = m0 + q * 32 + lane_id();      // output row of this thread
+      // warp-private transpose tile for the statistics, in front of the accumulator tile
+      float* s_tr = reinterpret_cast<float*>(smem) + warp * (32 * 33);
+      static_assert(L::ACC_OFF >= 4 * 32 * 33 * 4, "transpose tiles must fit in front of the accumulator tile");
       const bool row_ok = row < p.M;
       long long row_off;
       bool row_store = row_ok;
@@ -394,11 +379,19 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       } else {
         row_off = static_cast<long long>(row) * p.ldo;
       }
+      // split-K: the K slices of a tile add their partial sums in slice order (blockIdx.z) behind a turn counter, so the
+      // fp32 sums are the same every run; the last slice then owns the finished tile
+      uint32_t* turn = nullptr;
+      if ((p.epi == EPI_F32_ATOMIC || p.epi == EPI_F32_ATOMIC_T) && gridDim.z > 1) {
+        const uint32_t tix = blockIdx.x * gridDim.y + blockIdx.y;
+        turn = p.tile_counters != nullptr ? p.tile_counters + tix : p.det.ctr + DET_TURN_BASE + tix;
+        if (et == 0) turn_wait(turn, blockIdx.z);
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+      }
 #pragma unroll 1
       for (int c = 0; c < BLOCK_N; c += 32) {
         uint32_t v[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c, v);
-        tmem_ld_wait();
+        acc_ld32(s_acc, L::ACC_LD, q * 32 + lane_id(), c, v);
         if (et == 0 && c == 0) SLB_STAMP(11);
         const int col0 = n0 + c;
         if (p.epi == EPI_BF16) {
@@ -469,8 +462,10 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = static
               warp_col_sums_smem(s_tr, s1, c1, c2);
             }
             if (et == 0 && c == 0) SLB_STAMP(14);
-            atomicAdd(&s_stats[c + lane_id()], c1);
-            atomicAdd(&s_stats[BLOCK_N + c + lane_id()], c2);
+            for (int w = 0; w < 4; ++w) {                       // warps in order: a reproducible sum
+              if (warp == w) { s_stats[c + lane_id()] += c1; s_stats[BLOCK_N + c + lane_id()] += c2; }
+              asm volatile("bar.sync 1, 128;" ::: "memory");
+            }
           }
           if (et == 0 && c == 0) SLB_STAMP(15);
         } else if (p.epi == EPI_F32_ATOMIC) {
@@ -511,21 +506,18 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = __uint
           }
         }
       }
-      if (et == 0) SLB_STAMP(7);                               // TMEM drained / stores or reds issued
-      if (p.epi == EPI_F32_ATOMIC && p.tile_counters != nullptr) {
-        // ---- serial split-K tail: last slice of this tile finalises it ----
+      if (et == 0) SLB_STAMP(7);                               // accumulators drained / stores or reds issued
+      if (turn != nullptr) {
         __threadfence();
         if (et == 0) SLB_STAMP(8);                             // reds globally visible
-        asm volatile("bar.sync 1, 128;");
-        if (et == 0) {
-          const uint32_t tix = blockIdx.x * gridDim.y + blockIdx.y;
-          const uint32_t t = atomicAdd(p.tile_counters + tix, 1u);
-          const uint32_t last = (t == static_cast<uint32_t>(p.k_split) - 1u) ? 1u : 0u;
-          if (last) p.tile_counters[tix] = 0;
-          tmem_slot[1] = last;
-        }
-        asm volatile("bar.sync 1, 128;");
-        if (tmem_slot[1]) {
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        if (et == 0) turn_pass(turn, blockIdx.z, gridDim.z);
+      }
+      if (p.epi == EPI_F32_ATOMIC && p.tile_counters != nullptr) {
+        // ---- serial split-K tail: the last slice of this tile finalises it ----
+        if (et == 0) s_flag[1] = (gridDim.z == 1 || blockIdx.z == gridDim.z - 1) ? 1u : 0u;
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        if (s_flag[1]) {
           __threadfence();
 #pragma unroll 1
           for (int c = 0; c < BLOCK_N; c += 32) {
@@ -558,27 +550,27 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = __uint
                 for (int j = 0; j < 32; ++j) s1[j] = row_ok ? stored_value(f[j], static_cast<const T*>(nullptr)) : 0.f;
                 warp_col_sums_smem(s_tr, s1, c1, c2);
               }
-              atomicAdd(&s_stats[c + lane_id()], c1);
-              atomicAdd(&s_stats[BLOCK_N + c + lane_id()], c2);
+              for (int w = 0; w < 4; ++w) {                     // warps in order: a reproducible sum
+                if (warp == w) { s_stats[c + lane_id()] += c1; s_stats[BLOCK_N + c + lane_id()] += c2; }
+                asm volatile("bar.sync 1, 128;" ::: "memory");
+              }
             }
           }
         }
       }
-      if (want_stats && (p.epi == EPI_BF16 || tmem_slot[1])) {
-        asm volatile("bar.sync 1, 128;");
-        for (int i = et; i < BLOCK_N; i += 128) {
-          if (n0 + i < p.N) {
-            atomicAdd(p.col_sum + n0 + i, s_stats[i]);
-            atomicAdd(p.col_sumsq + n0 + i, s_stats[BLOCK_N + i]);
-          }
-        }
+      if (want_stats && (p.epi == EPI_BF16 || s_flag[1])) {
+        // one committing CTA per (m-tile, n-tile): the n-tile's column sums are added in m-tile order
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        det_commit<1>(p.det, blockIdx.y, blockIdx.x, gridDim.x, s_stats, 2 * BLOCK_N, p.col_sum + n0, BLOCK_N, p.col_sumsq + n0,
+                      et, 128);
       }
+      }  // epilogue warps
     }
   }
-  if (p.pub_flag != nullptr && warp >= 2 && my_iters > 0) {
+  if (p.pub_flag != nullptr && warp < 4 && my_iters > 0) {
     // ---- publish: every CTA fences its (peer) stores; the last one to arrive releases the mailbox flag system-wide ----
     asm volatile("bar.sync 1, 128;");
-    if (threadIdx.x == 64) {
+    if (threadIdx.x == 0) {
       __threadfence_system();
       const uint32_t t = atomicAdd(p.pub_ticket, 1u);
       if (t == gridDim.x * gridDim.y * gridDim.z - 1u) {
@@ -590,13 +582,8 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = __uint
       }
     }
   }
-  if (threadIdx.x == 64) SLB_STAMP(9);                         // epilogue thread 0 done
-  tc_fence_before();
+  if (threadIdx.x == 0) SLB_STAMP(9);                          // epilogue thread 0 done
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
-  }
   if (threadIdx.x == 0) SLB_STAMP(10);
 #undef SLB_STAMP
 }
@@ -644,8 +631,8 @@ static int make_tmap(CUtensorMap* m, const void* base, int rank, const uint64_t*
     es[i] = 1;
     if (i > 0) gstr[i - 1] = strides_bytes[i];
   }
-  // MN-major fp32 (tf32) operands must sit in the 32-byte-chunk swizzle (sm100.cuh umma_desc_sw128_base32)
-  const CUtensorMapSwizzle sw = (dtype == 1 && mn_major) ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B;
+  // MN-major fp32 (tf32) operands land unswizzled and are transposed in shared memory (sm90.cuh transpose_tf32_kmajor)
+  const CUtensorMapSwizzle sw = (dtype == 1 && mn_major) ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
   CUresult r = enc(m, tmap_dtype(dtype), rank, const_cast<void*>(base), gdim, gstr, bx, es,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -670,15 +657,20 @@ static int tmap_nhwc(CUtensorMap* m, const void* base, int B, int H, int W, int 
 }
 
 template <int MODE, int BN, typename T, bool BNB = false>
-static int launch(const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, dim3 grid, cudaStream_t st) {
+static int launch(const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p_in, dim3 grid, cudaStream_t st) {
   auto k = umma_gemm_kernel<MODE, BN, T, BNB>;
+  GemmParams p = p_in;
+  p.det = slb_det(st);
+  if (p.det.part == nullptr) return -30;
+  if (p.col_sum != nullptr && (grid.y > DET_TURN_BASE || (long long)grid.x * grid.y * 2 * BN > p.det.cap)) return -31;
+  if (grid.z > 1 && p.tile_counters == nullptr && (long long)grid.x * grid.y > DET_COUNTERS - DET_TURN_BASE) return -32;
   static bool attr_done = false;
   if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout<BN>::TOTAL);
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout<BN, T>::TOTAL);
     if (e != cudaSuccess) return -static_cast<int>(e) - 1000;
     attr_done = true;
   }
-  cudaError_t e0 = launch_k(k, grid, dim3(192), SmemLayout<BN>::TOTAL, st, a, b, p);
+  cudaError_t e0 = launch_k(k, grid, dim3(288), SmemLayout<BN, T>::TOTAL, st, a, b, p);
   if (e0 != cudaSuccess) return -static_cast<int>(e0) - 2000;
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : -static_cast<int>(e) - 2000;
@@ -688,7 +680,7 @@ template <int MODE>
 static int dispatch_bn(int bn, int dtype, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, dim3 grid,
                        cudaStream_t st) {
   using bf = __nv_bfloat16;
-  if (dtype == 1) {                               // fp32 tensors, kind::tf32 (conv fwd / dgrad / wgrad only)
+  if (dtype == 1) {                               // fp32 tensors, wgmma tf32 (conv fwd / dgrad / wgrad only)
     if constexpr (MODE == MODE_GEMM) return -5;
     else {
       if (p.bnb_y != nullptr) return -6;
@@ -756,7 +748,7 @@ int slb_preload_gemm() {
 // y[B,H,W,Cout] (pre-BN) = conv3x3(x[B,H,W,Cin], w[Cout][3][3][Cin]) + bias ; optional per-channel
 // sum / sum-of-squares accumulation (caller zeroes them).  flip=1 computes the input gradient:
 // x := dY [B,H,W,Cout_w], w as stored, out = dX[B,H,W,Cin_w]  (then Cin here means channels of A = Cout_w).
-// dtype: 0 = bf16 tensors (kind::f16), 1 = fp32 tensors (kind::tf32); x, w and y share it.
+// dtype: 0 = bf16 tensors (wgmma bf16), 1 = fp32 tensors (wgmma tf32); x, w and y share it.
 // block_n in {64,128,256} (0 = auto); k_split > 1 accumulates fp32 partial sums into `acc` ([M][Nout], zeroed by the
 // caller) with vector red.add instead of writing y — the last K slice of a tile (tile_counters) or slb_conv_finalize
 // then produces y.
@@ -881,7 +873,10 @@ int slb_conv3x3_wgrad(const void* x, const void* dy, float* dw, int B, int H, in
   p.M = ((rows + 127) / 128) * 128; p.N = Cin; p.k_iters = (pixels + KE - 1) / KE;   // tail pixels are TMA zero-fill
   const int m_tiles = p.M / 128, n_tiles = Cin / bn;
   if (k_split <= 0) {
-    k_split = (148 + m_tiles * n_tiles - 1) / (m_tiles * n_tiles);
+    int sms = 0, dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    k_split = (sms + m_tiles * n_tiles - 1) / (m_tiles * n_tiles);
     const int cap = p.k_iters / 4 > 1 ? p.k_iters / 4 : 1;      // keep >= 4 K iterations per CTA
     if (k_split > cap) k_split = cap;
     if (k_split < 1) k_split = 1;
@@ -922,6 +917,10 @@ int slb_gemm_bf16(const void* A, const void* Bm, float* out, int M, int N, int K
   if (k_split < 1) k_split = 1;
   if (k_split > p.k_iters) k_split = p.k_iters;
   if (epi == EPI_F32_STORE) k_split = 1;
+  {  // no empty K slices: every slice takes its turn
+    const int per = (p.k_iters + k_split - 1) / k_split;
+    k_split = (p.k_iters + per - 1) / per;
+  }
   p.k_split = k_split; p.a_mn = a_mn; p.b_mn = b_mn; p.epi = epi; p.out = out; p.ldo = ldo;
   dim3 grid((M + 127) / 128, (N + block_n - 1) / block_n, k_split);
   return dispatch_bn<MODE_GEMM>(block_n, 0, ta, tbm, p, grid, st);

@@ -1,4 +1,4 @@
-"""ctypes binding of ``_slb200.so`` — the hand-written sm_100a kernels.
+"""ctypes binding of ``_slb200.so`` — the hand-written sm_90a kernels.
 
 Every wrapper takes torch CUDA tensors (or raw device pointers), launches on the *current*
 torch stream (so it composes with CUDA-graph capture) and raises on a non-zero status.
@@ -50,7 +50,7 @@ def preload(device=None) -> None:
         bad = (lib().slb_preload_gemm() + lib().slb_preload_fused() + lib().slb_preload_elementwise()
                + lib().slb_preload_transformer() + lib().slb_preload_allreduce() + lib().slb_preload_ticket())
     if bad:
-        raise NativeError(f"{bad} kernels failed to load (wrong GPU architecture? this library is sm_100a only)")
+        raise NativeError(f"{bad} kernels failed to load (wrong GPU architecture? this library is sm_90a only)")
     _preloaded.add(d)
 
 
@@ -98,7 +98,7 @@ _TUNING = None
 
 
 def _tuning():
-    """Measured (BLOCK_N, split-K) table written by tools/tune_conv.py on a B200 (falls back to the heuristic)."""
+    """Measured (BLOCK_N, split-K) table written by tools/tune_conv.py (falls back to the heuristic when absent)."""
     global _TUNING
     if _TUNING is None:
         import json
@@ -138,8 +138,8 @@ def _ke(t) -> int:
 
 
 def conv3x3_fwd(x, w_bf16, y, bias=None, col_sum=None, col_sumsq=None, acc=None, tiling=None, counters=None):
-    """x [B,H,W,Cin], w [Cout,3,3,Cin] -> y [B,H,W,Cout] (pre-BN) + optional BN sums; x / w / y all bf16 (kind::f16)
-    or all fp32 (kind::tf32).  ``acc``: zeroed fp32 [M, Cout] scratch enabling split-K (the last K slice of a tile —
+    """x [B,H,W,Cin], w [Cout,3,3,Cin] -> y [B,H,W,Cout] (pre-BN) + optional BN sums; x / w / y all bf16 (wgmma bf16)
+    or all fp32 (wgmma tf32).  ``acc``: zeroed fp32 [M, Cout] scratch enabling split-K (the last K slice of a tile —
     or a finalize kernel — then produces y and the sums)."""
     B, H, W, Cin = x.shape
     Cout = w_bf16.shape[0]
@@ -253,7 +253,7 @@ def num_sms(device=None) -> int:
 def conv_bn_act_p2p(x, w_bf16, bias, gamma, beta, running_mean, running_var, nbt, save_mean, save_invstd, col_sum, col_sumsq,
                     y_opt, out, relu, pool, grid_bar, momentum=0.1, eps=1e-5, update_running=True, flag=None, seq=None,
                     hint=None):
-    """Fused cut-tail forward: conv3x3 -> batch stats -> grid barrier -> BN+ReLU(+pool) out of TMEM -> store into
+    """Fused cut-tail forward: conv3x3 -> batch stats -> grid barrier -> BN+ReLU(+pool) out of shared memory -> store into
     ``out`` (local or peer mailbox slot) -> publish flag.  ``y_opt``: optional local copy of the pre-BN output."""
     B, H, W, Cin = x.shape
     Cout = w_bf16.shape[0]
@@ -273,8 +273,8 @@ def fused_cut_supported(B, H, W, Cin, Cout, pool, ke: int = 64) -> bool:
         return False
     bn = 256 if Cout >= 256 else Cout
     total = ((B * H * W + 127) // 128) * (Cout // bn)
-    grid = min(total, 144)
-    return (total + grid - 1) // grid <= 512 // bn
+    grid = min(total, num_sms() - 4)                  # the persistent grid of slb_conv_bn_act_p2p
+    return (total + grid - 1) // grid <= (2 if bn <= 128 else 1)   # accumulator tiles per CTA that fit in shared memory
 
 
 # ------------------------------------------------------------------ memory-bound ops

@@ -1,6 +1,6 @@
-"""Autograd-visible wrappers of the token-model kernels (``csrc/transformer.cu`` + the tcgen05 GEMM).
+"""Autograd-visible wrappers of the token-model kernels (``csrc/transformer.cu`` + the wgmma GEMM).
 
-Each ``torch.autograd.Function`` below is one fused native op — forward *and* backward are hand-written sm_100a
+Each ``torch.autograd.Function`` below is one fused native op — forward *and* backward are hand-written sm_90a
 kernels; torch only keeps the tape.  Activations are bf16, parameters stay fp32 ``nn.Parameter``s (state-dict, FedAvg,
 LoRA and the flat fused optimizer are unchanged) and are read through a bf16 shadow: the one the flat optimizer
 refreshes inside its update kernel (``ops.optim``), or a cached cast for frozen parameters.  Weight / bias /
@@ -119,7 +119,7 @@ class _LinearFn(torch.autograd.Function):
         ldz = dzp.shape[1]
         if weight.requires_grad:
             tiles = ((n_out + 127) // 128) * ((k_in + 63) // 64)
-            ks = max(1, min((m + 63) // 64, 148 // max(tiles, 1)))
+            ks = max(1, min((m + 63) // 64, N.num_sms(dy.device) // max(tiles, 1)))
             # dW[n][k] += sum_t dz[t][n] x[t][k]     (both operands MN-major: token-major storage is the K axis)
             N.gemm_f32(dzp, x2, _grad_buf(weight).view(n_out, k_in), n_out, k_in, m, a_mn=True, b_mn=True, lda=ldz, ldb=k_in, ldo=k_in,
                        k_split=ks)

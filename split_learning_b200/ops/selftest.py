@@ -1,4 +1,4 @@
-"""Numerics self-test of every sm_100a kernel against plain PyTorch fp32 references.
+"""Numerics self-test of every sm_90a kernel against plain PyTorch fp32 references.
 
     python -m split_learning_b200.ops.selftest            # all checks, each in its own process
     python -m split_learning_b200.ops.selftest NAME ...   # selected checks, in-process
@@ -36,7 +36,7 @@ def _bf(x):
 
 
 BF, F32 = torch.bfloat16, torch.float32
-DTYPES = (F32, BF)          # fp32 tensors = tcgen05 kind::tf32 (parity mode), bf16 = kind::f16 (fast mode)
+DTYPES = (F32, BF)          # fp32 tensors = wgmma tf32 (parity mode), bf16 = wgmma bf16 (fast mode)
 
 
 def _exact():

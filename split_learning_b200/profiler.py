@@ -58,7 +58,7 @@ def profile_speed(model_name: str, batch: int = 4, data_name: Optional[str] = No
                   device: Optional[str] = None, train: Optional[bool] = None) -> Dict:
     """Whole-model throughput only — the FLEX profiler (other/FLEX/profiling.py:23-92): BERT-like models time a full
     training step (forward of the mean, backward, AdamW), CNNs a forward pass; returns ``{"speed": samples/s}``.
-    The step runs through the stage executor, i.e. the native sm_100a path on CUDA."""
+    The step runs through the stage executor, i.e. the native sm_90a path on CUDA."""
     from .train.executor import make_executor
     device = device or ("cuda" if torch.cuda.is_available() else "cpu")
     klass = get_model_class(model_name, data_name)

@@ -1,13 +1,13 @@
-"""Native sm_100a stage executor for VGG-family layer tables.
+"""Native sm_90a stage executor for VGG-family layer tables.
 
 A stage's ``LayerSpec`` slice is compiled into a static plan of fused blocks
 
-    ConvBlock   = [conv3x3] [BatchNorm2d(train)] [ReLU] [MaxPool2]     (tcgen05 implicit GEMM
+    ConvBlock   = [conv3x3] [BatchNorm2d(train)] [ReLU] [MaxPool2]     (wgmma implicit GEMM
                   + fused BN-stat epilogue; BN/ReLU/pool apply kernel writes the block output —
                   for the last block of a non-last stage that output pointer *is* the next
                   stage's mailbox slot, local or NVLink-peer, and the kernel publishes the flag)
     Dropout     = standalone dropout on a dense activation (VGG layer 46)
-    LinearBlock = Linear [ReLU] [Dropout]   (swap-AB tcgen05 GEMM, split-K, fused finalisation)
+    LinearBlock = Linear [ReLU] [Dropout]   (swap-AB wgmma GEMM, split-K, fused finalisation)
 
 over flat fp32 master / gradient / momentum buffers.  Forward, backward(+recompute) and the
 optimizer step of one microbatch are captured once per batch size into CUDA graphs; the host
@@ -16,13 +16,13 @@ only copies the input in and replays.
 Two compute precisions (``precision=`` / ``b200.precision`` / ``SLB200_PRECISION``):
 
 * ``tf32`` (default, the reference's precision): fp32 activations and weights end to end,
-  convolutions on ``tcgen05.mma kind::tf32`` with fp32 accumulation (what PyTorch/cuDNN does by
+  convolutions on ``wgmma`` tf32 with fp32 accumulation (what PyTorch/cuDNN does by
   default for the reference's ``nn.Conv2d``), Linear layers in IEEE fp32 on the CUDA cores (the
   reference's ``nn.Linear`` is an fp32 cuBLAS GEMM) with the SGD-momentum step fused into the
   weight-gradient pass; BN / ReLU / pool / CE / SGD in fp32.  No reduced-precision copy of
   anything exists in this mode.
 * ``bf16`` (opt-in fast mode): bf16 activations and a bf16 weight shadow refreshed by the fused
-  SGD kernel, ``kind::f16`` tensor-core GEMMs for convolutions and Linear layers.
+  SGD kernel, bf16 wgmma GEMMs for convolutions and Linear layers.
 
 Semantics follow the reference trainer (src/train/VGG16.py:61-190): SGD(lr, momentum) step per
 microbatch, recompute-forward with *current* weights on non-last stages (BN running stats
@@ -132,7 +132,7 @@ def compile_plan(model: SplitModel):
                 i += 1
             b.cout = c
             if b.conv is not None and b.cin > 4 and (b.cin % 64 or b.cout % 64):
-                raise NotImplementedError("tcgen05 conv path needs channels % 64 == 0")
+                raise NotImplementedError("wgmma conv path needs channels % 64 == 0")
             if b.conv is not None and b.bn is None and (b.relu or b.pool):
                 raise NotImplementedError("conv+ReLU/pool without BatchNorm has no native plan yet")
             if b.conv is not None and b.bn is None and b.cin <= 4:

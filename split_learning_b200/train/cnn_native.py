@@ -4,12 +4,12 @@ dense 3x3 convs with stride 1 or 2, 1x1 convs, 32-channel layers, one max-pool, 
 
 Same scheme as ``token_native``: the module tree (parameter names, state-dict, checkpoints) is untouched, the stage's
 ``forward`` is re-bound to a small NHWC/bf16 program whose heavy ops are ``torch.autograd.Function``s over the
-hand-written sm_100a kernels:
+hand-written sm_90a kernels:
 
-* 3x3 conv  -> the tcgen05 implicit-GEMM kernel (forward, dgrad with mirrored taps, split-K wgrad).  Channel counts
+* 3x3 conv  -> the wgmma implicit-GEMM kernel (forward, dgrad with mirrored taps, split-K wgrad).  Channel counts
   that are not multiples of 64 are zero-padded in the bf16 weight view; stride 2 is computed at stride 1 and
   sub-sampled (4 of the 27 convs), its backward scatters into a zero tensor;
-* 1x1 conv  -> the tcgen05 GEMM of ``ops.nn.linear`` on the NHWC view (no im2col, no layout change);
+* 1x1 conv  -> the wgmma GEMM of ``ops.nn.linear`` on the NHWC view (no im2col, no layout change);
 * first conv (Cin = 1 or 3, NCHW fp32 input) -> ``conv3x3_small_fwd_kernel`` / ``conv3x3_small_wgrad_kernel``;
 * BatchNorm(train) + ReLU (+ MaxPool2) -> ``col_stats`` + ``bn_relu_pool_fwd`` / ``bn_relu_pool_bwd`` (running
   statistics and ``num_batches_tracked`` updated by the kernel);

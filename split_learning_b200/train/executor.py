@@ -5,7 +5,7 @@
     CPU (tests, plumbing config #1), for model families that do not yet have a native
     plan, and as the numerics oracle.
   * ``B200Executor``   — (``b200_executor.py``) VGG-family stages compiled to hand-written
-    sm_100a kernels + CUDA graphs; selected automatically on CUDA.
+    sm_90a kernels + CUDA graphs; selected automatically on CUDA.
 
 Reference semantics preserved (SURVEY §3.3/§3.4):
   * non-last stages *recompute* the forward with current weights when the gradient comes
@@ -34,7 +34,7 @@ def make_optimizer(model: nn.Module, model_name: str, learning: dict, shadow: bo
     lr = float(learning.get("learning-rate", 0.01))
     adamw = model_name.upper() in _ADAMW_MODELS
     if params and params[0].is_cuda:
-        # CUDA: one flat buffer + the fused sm_100a optimizer kernels (no silent fallback: a missing library raises)
+        # CUDA: one flat buffer + the fused sm_90a optimizer kernels (no silent fallback: a missing library raises)
         from ..ops.optim import FlatFusedOptimizer
         return FlatFusedOptimizer(params, "adamw" if adamw else "sgd", lr=lr, momentum=float(learning.get("momentum", 0.0)),
                                   weight_decay=float(learning.get("weight-decay", 0.01)), shadow=shadow)
@@ -66,7 +66,7 @@ class TorchExecutor(StageExecutor):
                  graphs: bool = False):
         self.model = model.to(device)       # parameters must sit on the device before the optimizer re-homes them
         self.native = bool(native)
-        if self.native:                     # blocks -> fused sm_100a ops (train/token_native.py, train/cnn_native.py)
+        if self.native:                     # blocks -> fused sm_90a ops (train/token_native.py, train/cnn_native.py)
             from . import cnn_native, token_native
             (cnn_native if cnn_native.supports(self.model) else token_native).nativize(self.model)
         self.model_name = model_name
@@ -256,7 +256,7 @@ class TorchExecutor(StageExecutor):
 
 def make_executor(model: SplitModel, model_name: str, learning: dict, device, is_first: bool, is_last: bool,
                   b200_opts: Optional[dict] = None) -> StageExecutor:
-    """Pick the executor: native sm_100a plan on CUDA for supported tables, torch otherwise."""
+    """Pick the executor: native sm_90a plan on CUDA for supported tables, torch otherwise."""
     opts = b200_opts or {}
     kind = opts.get("executor", "auto")
     dev = torch.device(device)
@@ -280,6 +280,6 @@ def make_executor(model: SplitModel, model_name: str, learning: dict, device, is
                                  recompute=bool(opts.get("recompute", True)), clip_grad_norm=clip, native=True,
                                  graphs=bool(opts.get("token-graphs", True)))
         if kind == "b200":
-            raise RuntimeError(f"no native sm_100a plan for {type(model).__name__}")
+            raise RuntimeError(f"no native sm_90a plan for {type(model).__name__}")
     return TorchExecutor(model, model_name, learning, device=dev, is_first=is_first, is_last=is_last,
                          recompute=bool(opts.get("recompute", True)), clip_grad_norm=clip)

@@ -1,7 +1,7 @@
 """Native execution of the token-model families (KWT / ViT / BERT_AGNEWS / BERT_EMOTION, with or without LoRA).
 
-``nativize(model)`` re-binds the ``forward`` of every block of a stage to the fused sm_100a ops of ``ops.nn``
-(tcgen05 GEMMs with bias / GELU / tanh / residual epilogues, tcgen05 attention, LayerNorm with fused
+``nativize(model)`` re-binds the ``forward`` of every block of a stage to the fused sm_90a ops of ``ops.nn``
+(wgmma GEMMs with bias / GELU / tanh / residual epilogues, wgmma attention, LayerNorm with fused
 dropout+residual, hash dropout, embedding gather) while leaving the module tree — and therefore parameter names,
 state-dicts, checkpoints, LoRA wrapping / merging and FedAvg — untouched.  The reference runs these layers through
 stock ``torch.nn`` (src/model/BERT_AGNEWS.py:56-165, src/model/KWT_SPEECHCOMMANDS.py:5-109,

@@ -1,4 +1,3 @@
-import importlib
 import os
 import sys
 
@@ -8,11 +7,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 os.environ.setdefault("SLB200_QUIET", "1")
-REFERENCE = "/root/reference"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "slow: long-running")
 
 
@@ -24,21 +22,3 @@ def pytest_collection_modifyitems(config, items):
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)
-
-
-def import_reference(module: str, root: str = REFERENCE):
-    """Import a module of the read-only reference tree as a numerics/behaviour oracle."""
-    if not os.path.isdir(root):
-        pytest.skip("reference tree not mounted")
-    for k in [k for k in sys.modules if k == "src" or k.startswith("src.")]:
-        del sys.modules[k]
-    sys.path.insert(0, root)
-    try:
-        return importlib.import_module(module)
-    finally:
-        sys.path.remove(root)
-
-
-@pytest.fixture
-def ref():
-    return import_reference

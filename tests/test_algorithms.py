@@ -8,25 +8,18 @@ from split_learning_b200.fedavg import fedasync_merge, fedavg_state_dicts
 from split_learning_b200.models import VGG16_CIFAR10
 from split_learning_b200.planning import auto_threshold, clustering_algorithm, gmm_1d, kmeans, partition, partition_multi
 
+from oracle_cases import CLUSTER_SEED, PARTITION_CASES, SELECTION_SEED, as_tensor, fedavg_inputs, layout_digest, load_json
 
-def _rand_sd(seed, keys=("a", "b", "n"), nan=False):
-    g = torch.Generator().manual_seed(seed)
-    sd = {"a": torch.randn(4, 3, generator=g), "b": torch.randn(5, generator=g),
-          "n": torch.tensor(seed * 3 + 1, dtype=torch.int64)}
-    if nan:
-        sd["a"][0, 0] = float("nan")
-    return {k: sd[k] for k in keys}
+# answers of the reference implementation (src/Utils.py, src/Partition.py, src/Cluster.py, src/Selection.py) on the same
+# inputs, recorded by tools/make_golden.py
+ORACLE = load_json("algorithms.json")
 
 
-def test_fedavg_matches_reference(ref):
-    theirs = ref("src.Utils").fedavg_state_dicts if False else None
-    # src.Utils imports pika at module import; re-implement the oracle call through a stub
-    import sys, types
-    sys.modules.setdefault("pika", types.ModuleType("pika"))
-    theirs = ref("src.Utils").fedavg_state_dicts
-    dicts = [_rand_sd(1), _rand_sd(2, nan=True), _rand_sd(3, keys=("a", "n"))]
+def test_fedavg_matches_reference():
+    dicts = fedavg_inputs()
     for w in (None, [3, 1, 7]):
-        mine, oracle = fedavg_state_dicts(dicts, w), theirs(dicts, w)
+        mine = fedavg_state_dicts(dicts, w)
+        oracle = {k: as_tensor(v) for k, v in ORACLE["fedavg"][str(w)].items()}
         assert set(mine) == set(oracle)
         for k in mine:
             assert mine[k].dtype == oracle[k].dtype
@@ -47,16 +40,11 @@ def test_fedasync():
     assert torch.equal(fedasync_merge(None, n, 0.5)["w"], n["w"])
 
 
-def test_partition_matches_reference(ref):
-    theirs = ref("src.Partition").partition
-    rng = np.random.RandomState(0)
-    for _ in range(20):
-        L = rng.randint(3, 30)
-        e1 = [list(rng.rand(L) + 0.01) for _ in range(rng.randint(1, 4))]
-        e2 = [list(rng.rand(L) * 0.3 + 0.01) for _ in range(rng.randint(1, 4))]
-        n1, n2 = list(rng.rand(len(e1)) + 0.1), list(rng.rand(len(e2)) + 0.1)
-        size = list(rng.rand(L) * 5)
-        assert partition(e1, n1, e2, n2, size) == theirs(e1, n1, e2, n2, size)
+def test_partition_matches_reference():
+    cases = PARTITION_CASES()
+    assert len(cases) == len(ORACLE["partition"]) == 20
+    for case, theirs in zip(cases, ORACLE["partition"]):
+        assert partition(*case) == theirs
 
 
 def test_partition_multi():
@@ -66,23 +54,21 @@ def test_partition_multi():
     assert partition_multi(e[:2], [[1e9]] * 2, [1.0] * 12) == partition(e[0], [1e9], e[1], [1e9], [1.0] * 12)
 
 
-def test_clustering_matches_reference(ref):
-    theirs = ref("src.Cluster").clustering_algorithm
-    rng = np.random.RandomState(1)
+def test_clustering_matches_reference():
+    rng = np.random.RandomState(CLUSTER_SEED)
     a = np.concatenate([rng.dirichlet([10, 1, 1, 1], 6), rng.dirichlet([1, 1, 10, 10], 5)]) * 500
     lm, im = clustering_algorithm(a, 2)
-    lt, it = theirs(a, 2)
-    assert (np.asarray(lm) == np.asarray(lt)).all() and im == [[int(x[0])] for x in it]
+    lt = ORACLE["clustering"]["labels"]
+    assert (np.asarray(lm) == np.asarray(lt)).all() and im == ORACLE["clustering"]["infos"]
     # dependency-free path finds the same partition (up to relabelling)
     lk, _ = kmeans(a / a.sum(1, keepdims=True), 2)
     assert len(set(zip(lk.tolist(), np.asarray(lt).tolist()))) == 2
 
 
-def test_selection_threshold(ref):
-    theirs = ref("src.Selection").auto_threshold
-    rng = np.random.RandomState(2)
+def test_selection_threshold():
+    rng = np.random.RandomState(SELECTION_SEED)
     perf = np.concatenate([rng.normal(100, 5, 12), rng.normal(1000, 40, 10)]).clip(1)
-    t_mine, t_ref = auto_threshold(perf), theirs(perf)
+    t_mine, t_ref = auto_threshold(perf), ORACLE["selection_threshold"]
     assert abs(np.log(t_mine) - np.log(t_ref)) < 1e-6
     t_own = auto_threshold(perf, backend="own")
     assert 130 < t_own < 800 and abs(np.log(t_own) - np.log(t_ref)) < 0.35
@@ -100,7 +86,7 @@ def test_label_counts():
     assert r.shape == (2, 10) and r.sum() <= 2000 and r.max() > r.min()
 
 
-def test_checkpoint_slice_merge_roundtrip(tmp_path, ref):
+def test_checkpoint_slice_merge_roundtrip(tmp_path):
     torch.manual_seed(0)
     full = VGG16_CIFAR10().state_dict()
     p = str(tmp_path / "VGG16_CIFAR10.pth")
@@ -109,9 +95,10 @@ def test_checkpoint_slice_merge_roundtrip(tmp_path, ref):
     parts = [slice_for_stage(loaded, "VGG16", "CIFAR10", l) for l in ([0, 5], [5, 10], [10, -1])]
     merged = merge_stages(parts)
     assert set(merged) == set(full) and all(torch.equal(merged[k], full[k]) for k in full)
-    # the reference's own class can load our checkpoint (layout compatibility)
-    theirs = ref("src.model.VGG16_CIFAR10").VGG16_CIFAR10()
-    theirs.load_state_dict(torch.load(p, weights_only=True))
+    # the reference's own class can load our checkpoint (layout compatibility): the strict load_state_dict check against
+    # the reference model's recorded keys, shapes and dtypes
+    theirs = load_json("models.json")["layouts"]["VGG16_CIFAR10"][f"0,{VGG16_CIFAR10.num_layers()}"]
+    assert layout_digest(torch.load(p, weights_only=True)) == theirs
     assert load_checkpoint(str(tmp_path / "missing.pth")) is None
 
 

@@ -1,29 +1,31 @@
-import glob
-
 import pytest
 import yaml
 
 from split_learning_b200.config import load_config, normalize
 from split_learning_b200.plan import rank_assignment, resolve_range, stage_layers
 
+from oracle_cases import reference_config
 
-@pytest.mark.parametrize("path", ["/root/reference/config.yaml"] + sorted(glob.glob("/root/reference/other/*/config.yaml")))
-def test_reference_configs_load_and_roundtrip(path):
-    cfg = load_config(path)
+# the reference's config.yaml and other/<variant>/config.yaml, stored under tests/golden/reference_configs
+
+
+@pytest.mark.parametrize("name", ["main", "2LS", "Cluster_FSL", "DCSL", "FLEX", "Vanilla_SL"])
+def test_reference_configs_load_and_roundtrip(name):
+    cfg = load_config(reference_config(name))
     again = normalize(cfg.to_dict())
     assert again.to_dict() == cfg.to_dict()
     assert cfg.learning["batch-size"] > 0 and "control-count" in cfg.learning
 
 
 def test_variant_keys():
-    flex = load_config("/root/reference/other/FLEX/config.yaml")
+    flex = load_config(reference_config("FLEX"))
     assert flex.cluster_mode and flex.num_cluster == 3 and flex.cluster_cut_layers == [[7], [7], [4]]
     assert (flex.t_g, flex.t_c, flex.select_ratio) == (4, 2, 0.5)
-    two = load_config("/root/reference/other/2LS/config.yaml")
+    two = load_config(reference_config("2LS"))
     assert two.cluster_cut_layers == [[2]] * 3 and two.infor_cluster == [[2, 1]] * 3 and two.warnings
-    dcsl = load_config("/root/reference/other/DCSL/config.yaml")
+    dcsl = load_config(reference_config("DCSL"))
     assert dcsl.local_round == 1 and dcsl.no_cluster_cut_layers == [7]
-    van = load_config("/root/reference/other/Vanilla_SL/config.yaml")
+    van = load_config(reference_config("Vanilla_SL"))
     assert van.limited_time == {"enable": False, "epoch": 10, "time": 10.0}
     assert van.learning["clip-grad-norm"] == 0.0
 

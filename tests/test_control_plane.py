@@ -12,6 +12,8 @@ from split_learning_b200.runner import DEFAULT_PROFILE, run_inproc
 from split_learning_b200.transport import InProcBroker, TcpBroker, TcpChannel
 from split_learning_b200.transport.broker import delete_old_queues
 
+from oracle_cases import reference_config
+
 
 def test_inproc_broker_fifo_and_blocking_get():
     b = InProcBroker()
@@ -68,7 +70,7 @@ def test_message_schemas_match_reference_fields():
 
 
 def _auto_cfg(tmp_path, selection):
-    raw = yaml.safe_load(open("/root/reference/config.yaml"))
+    raw = yaml.safe_load(open(reference_config()))
     raw["server"].update({"clients": [4, 2], "auto-mode": True, "validation": False, "global-round": 1})
     raw["server"]["data-distribution"].update({"non-iid": True, "num-sample": 64})
     raw["server"]["cluster-selection"] = {"num-cluster": 2, "algorithm-cluster": "KMeans", "selection-mode": selection}

@@ -14,12 +14,13 @@ from split_learning_b200.config import normalize
 from split_learning_b200.models import VGG16_CIFAR10
 from split_learning_b200.runner import run_inproc
 
+from oracle_cases import reference_config
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _raw(tmp, clients=(1, 1), cut=(7,), rounds=1, samples=64, **server):
-    raw = yaml.safe_load(open("/root/reference/config.yaml")) if os.path.exists("/root/reference/config.yaml") \
-        else yaml.safe_load(open(os.path.join(ROOT, "config.yaml")))
+    raw = yaml.safe_load(open(reference_config()))
     raw["server"].update({"clients": list(clients), "global-round": rounds, "validation": True})
     raw["server"]["manual"]["no-cluster"]["cut-layers"] = list(cut)
     raw["server"]["data-distribution"]["num-sample"] = samples

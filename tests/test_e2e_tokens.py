@@ -1,6 +1,6 @@
 """Token-model families (and MobileNetv1) through the full control plane (REGISTER .. STOP): KWT / ViT with AdamW, BERT with LoRA
 wrapping + merge before upload (reference src/RpcClient.py:61-66,99-103,121-122).  CPU: torch executor; GPU: the
-native sm_100a blocks (``train/token_native.py``) — same config, same checkpoint layout."""
+native sm_90a blocks (``train/token_native.py``) — same config, same checkpoint layout."""
 import os
 
 import pytest

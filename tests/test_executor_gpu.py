@@ -222,6 +222,37 @@ def test_device_pipeline_matches_tensor_api():
     assert _cos(w2, w1) > 0.999
 
 
+@pytest.mark.parametrize("precision", ["tf32", "bf16"])
+def test_pipeline_is_bitwise_reproducible(precision):
+    """Two pipelines built from the same seed and fed the same microbatches (control-count 3, dropout on, the layers with
+    split-K, BatchNorm statistics and K-sliced Linear kernels) produce bit-identical losses, cut activations and weights:
+    no sum depends on the order in which blocks finish."""
+    from split_learning_b200.models import VGG16_CIFAR10
+    from split_learning_b200.parallel.pipeline import LocalPipeline
+    from split_learning_b200.train.b200_executor import B200Executor
+    dev = torch.device("cuda:0")
+    learning = dict(LEARNING, precision=precision)
+    g = torch.Generator().manual_seed(4)
+    data = [(torch.randn(32, 3, 32, 32, generator=g).pin_memory(), torch.randint(0, 10, (32,), generator=g).pin_memory())
+            for _ in range(12)]
+    runs = []
+    for _ in range(2):
+        torch.manual_seed(0)
+        exs = [B200Executor(VGG16_CIFAR10(0, 7), "VGG16", learning, dev, is_first=True),
+               B200Executor(VGG16_CIFAR10(7, 52), "VGG16", learning, dev, is_last=True)]
+        pipe = LocalPipeline(exs, 32, 3)
+        losses = []
+        for x, y in data:
+            pipe.run([(x, y)])
+            pipe.synchronize()
+            losses.append(float(pipe.loss()[0]))
+        act = pipe.stages[0].fwd_out.payload[(len(data) - 1) % 3].float().cpu()
+        runs.append((losses, act, exs[0].P.detach().cpu(), exs[1].P.detach().cpu()))
+    (la, aa, p1a, p2a), (lb, ab, p1b, p2b) = runs
+    assert la == lb
+    assert torch.equal(aa, ab) and torch.equal(p1a, p1b) and torch.equal(p2a, p2b)
+
+
 def test_smoke_entry():
     import __graft_entry__ as ge
     ge.smoke()
@@ -372,7 +403,7 @@ def test_launch_py_device_plane_across_processes(tmp_path):
     ("vanilla_sl", (2, 1), [dict(layer_id=1), dict(layer_id=1), dict(layer_id=2)], {}),
 ])
 def test_host_plane_with_native_executor_on_gpu(tmp_path, algo, clients, specs, extra):
-    """Broker data plane (pickled CPU arrays, any topology/variant) driving the native sm_100a stage executor through its
+    """Broker data plane (pickled CPU arrays, any topology/variant) driving the native sm_90a stage executor through its
     tensor API: competing consumers (2:1), DCSL's SDA batch concatenation (B = 64 on the last stage), sequential hand-off."""
     import yaml
     from split_learning_b200.checkpoint import load_checkpoint

@@ -1,4 +1,4 @@
-"""Every sm_100a kernel against a plain PyTorch fp32 reference (run on the B200 box)."""
+"""Every sm_90a kernel against a plain PyTorch fp32 reference (needs an H100)."""
 import pytest
 import torch
 

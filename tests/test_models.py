@@ -1,43 +1,36 @@
 import pytest
 import torch
 
+from oracle_cases import layout_digest, load_json, model_cases
+
 from split_learning_b200.models import (BERT_AGNEWS, BERT_EMOTION, KWT_SPEECHCOMMANDS, MobileNetv1_CIFAR10,
                                         VGG16_CIFAR10, VGG16_MNIST, ViT_CIFAR10, ViT_MNIST, build_stage,
                                         get_model_class)
 from split_learning_b200.models.lora import apply_lora, merge_lora
 
-VAN = "/root/reference/other/Vanilla_SL"
-CASES = [
-    (VGG16_CIFAR10, "src.model.VGG16_CIFAR10", "VGG16_CIFAR10", "/root/reference"),
-    (KWT_SPEECHCOMMANDS, "src.model.KWT_SPEECHCOMMANDS", "KWT_SPEECHCOMMANDS", "/root/reference"),
-    (BERT_AGNEWS, "src.model.BERT_AGNEWS", "BERT_AGNEWS", "/root/reference"),
-    (VGG16_MNIST, "src.model.VGG16_MNIST", "VGG16_MNIST", VAN),
-    (MobileNetv1_CIFAR10, "src.model.MobileNetv1_CIFAR10", "MobileNetv1_CIFAR10", VAN),
-    (ViT_CIFAR10, "src.model.ViT_CIFAR10", "ViT_CIFAR10", VAN),
-    (ViT_MNIST, "src.model.ViT_MNIST", "ViT_MNIST", VAN),
-    (BERT_EMOTION, "src.model.BERT_EMOTION", "BERT_EMOTION", VAN),
-]
+# state-dict layouts and forward outputs of the reference model classes (src/model/*.py, other/Vanilla_SL/src/model/*.py),
+# recorded by tools/make_golden.py
+ORACLE = load_json("models.json")
+CASES = [(c[0], c[2]) for c in model_cases()]
 
 
-@pytest.mark.parametrize("mine,mod,cls,root", CASES, ids=[c[2] for c in CASES])
-def test_state_dict_keys_match_reference(ref, mine, mod, cls, root):
-    theirs = getattr(ref(mod, root), cls)
+@pytest.mark.parametrize("mine,cls", CASES, ids=[c[1] for c in CASES])
+def test_state_dict_keys_match_reference(mine, cls):
     n = mine.num_layers()
     for a, b in [(0, n), (0, 3), (3, n), (2, 5)]:
-        sa, sb = mine(a, b).state_dict(), theirs(start_layer=a, end_layer=b).state_dict()
-        assert list(sa) == list(sb)
-        for k in sa:
-            assert sa[k].shape == sb[k].shape and sa[k].dtype == sb[k].dtype
+        # same keys in the same order, same shapes and dtypes (stored as a digest of the reference's list)
+        assert layout_digest(mine(a, b).state_dict()) == ORACLE["layouts"][cls][f"{a},{b}"], (cls, a, b)
 
 
-@pytest.mark.parametrize("mine,mod,cls,root", [CASES[0], CASES[1], CASES[5]], ids=["VGG16", "KWT", "ViT"])
-def test_forward_matches_reference(ref, mine, mod, cls, root):
-    theirs = getattr(ref(mod, root), cls)
-    m, t = mine().eval(), theirs().eval()
-    m.load_state_dict(t.state_dict())
+@pytest.mark.parametrize("mine,cls", [CASES[0], CASES[1], CASES[5]], ids=["VGG16", "KWT", "ViT"])
+def test_forward_matches_reference(mine, cls):
+    # the recorded outputs are the reference model's, run with the weights our class draws under seed 0
+    torch.manual_seed(0)
+    m = mine().eval()
+    torch.manual_seed(1)
     x = mine.example_input(2)
     with torch.no_grad():
-        assert torch.allclose(m(x), t(x), atol=1e-5)
+        assert torch.allclose(m(x), torch.tensor(ORACLE["forward"][cls]), atol=1e-5)
 
 
 def test_vgg16_table_facts():

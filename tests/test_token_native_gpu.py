@@ -1,4 +1,4 @@
-"""Token-model kernels (ops/csrc/transformer.cu + tcgen05 GEMM epilogues) against plain PyTorch fp32 references,
+"""Token-model kernels (ops/csrc/transformer.cu + wgmma GEMM epilogues) against plain PyTorch fp32 references,
 then whole KWT / ViT / BERT stages through ``nativize`` against the stock torch modules."""
 import math
 

@@ -10,8 +10,6 @@ from split_learning_b200.checkpoint import load_checkpoint
 from split_learning_b200.config import normalize
 from split_learning_b200.runner import run_variant
 
-REF = "/root/reference/other"
-
 
 def _base(tmp, algo, clients, **server):
     raw = {"server": {"global-round": 1, "clients": list(clients), "no-cluster": {"cut-layers": [7]}, "model": "VGG16",

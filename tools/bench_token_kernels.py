@@ -1,6 +1,6 @@
-"""Isolated timings + roofline fractions of the token-model kernels (tcgen05 GEMM epilogues, LayerNorm, attention).
+"""Isolated timings + roofline fractions of the token-model kernels (wgmma GEMM epilogues, LayerNorm, attention).
 
-    python tools/bench_token_kernels.py [--out profiles/kernels_tokens_r1.json]
+    python tools/bench_token_kernels.py [--out profiles/kernels_tokens.json]
 
 L2 is flushed between iterations (a 256 MB write); CUDA events; fractions are of MEASURED_PEAKS.json (cuBLAS bf16 burst,
 HBM copy bandwidth).
@@ -41,7 +41,7 @@ def main():
     a = ap.parse_args()
     N.require()
     N.preload()
-    peaks = {"bf16_tflops": 1703.6, "hbm_gbs": 6482.7}
+    peaks = {"bf16_tflops": 989.0, "hbm_gbs": 3350.0}          # H100 SXM data sheet unless MEASURED_PEAKS.json exists
     try:
         mp = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))
         peaks["bf16_tflops"] = float(mp.get("bf16_tflops_burst", mp.get("bf16_tflops", peaks["bf16_tflops"])))
@@ -74,7 +74,7 @@ def main():
                      "tflops": round(fl / us / 1e6, 1), "frac_bf16_peak": round(fl / us / 1e6 / peaks["bf16_tflops"], 3)})
         dw = torch.zeros(n, k, device="cuda")
         tiles = ((n + 127) // 128) * ((k + 63) // 64)
-        ks = max(1, min((tokens + 63) // 64, 148 // max(tiles, 1)))
+        ks = max(1, min((tokens + 63) // 64, N.num_sms() // max(tiles, 1)))
         us = timeit(lambda: N.gemm_f32(dz, x, dw, n, k, tokens, a_mn=True, b_mn=True, lda=n, ldb=k, ldo=k, k_split=ks))
         rows.append({"kernel": "umma_gemm<MODE_GEMM> ffn1 wgrad (both MN-major, fp32 red.add)", "tokens": tokens, "N": k, "K": tokens,
                      "us": round(us, 1), "tflops": round(fl / us / 1e6, 1),

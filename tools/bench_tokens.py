@@ -1,4 +1,4 @@
-"""Step time of the token-model families and MobileNetv1, native sm_100a ops vs stock torch modules (same executor, same optimizer).
+"""Step time of the token-model families and MobileNetv1, native sm_90a ops vs stock torch modules (same executor, same optimizer).
 
     python tools/bench_tokens.py [--steps 30] [--warmup 10]
 

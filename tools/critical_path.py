@@ -3,7 +3,7 @@ the dependent chain of the stage-2 program (main stream) against the forked weig
 stage-1 streams.  Durations are ncu's serialized per-kernel times (no overlap, launch ramp included), so the sums are an
 upper bound of the in-graph time of each chain.
 
-    python tools/critical_path.py gpurun_out/r2_launches_tf32_final.csv --per-step 117 > profiles/r2/critical_path_tf32.md
+    python tools/critical_path.py launches_tf32.csv --per-step 117 > profiles/critical_path_tf32.md
 """
 import argparse
 import collections
@@ -56,7 +56,7 @@ def main():
     cats = collections.Counter()
     for i, (k, us) in enumerate(by_stream[main_stream]):
         run += us
-        cat = ("conv GEMM (tcgen05)" if k.startswith("umma_gemm") else "Linear (fp32 CUDA cores)" if k.startswith("linear_") else
+        cat = ("conv GEMM (wgmma)" if k.startswith("umma_gemm") else "Linear (fp32 CUDA cores)" if k.startswith("linear_") else
                "BatchNorm" if k.startswith("bn_") else "other")
         cats[cat] += us
         print(f"| {i} | `{k}` | {us:.2f} | {run:.1f} |")

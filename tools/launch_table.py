@@ -1,7 +1,7 @@
 """ncu launch list (``--metrics gpu__time_duration.sum --csv``) -> markdown: per-kernel totals and the ordered kernel
 sequence of one training step with its stream — what the F / L / B programs are made of.
 
-    python tools/launch_table.py gpurun_out/r2_launches_tf32.csv --steps 3 > profiles/r2/launches_tf32.md
+    python tools/launch_table.py launches_tf32.csv --steps 3 > profiles/launches_tf32.md
 """
 import argparse
 import collections

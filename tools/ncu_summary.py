@@ -1,6 +1,6 @@
 """Summarise an .ncu-rep (read on the CPU box) into markdown: key raw metrics + top stall instructions.
 
-    python tools/ncu_summary.py gpurun_out/prof_fused.ncu-rep profiles/ncu_fused_cut7.md "title"
+    python tools/ncu_summary.py prof_fused.ncu-rep profiles/ncu_fused_cut7.md "title"
 """
 import csv
 import io
@@ -47,8 +47,8 @@ def main(rep, dst, title):
         tot = sum(n for n, _ in rows) or 1
         sass = " ".join(s for _, s in rows)
         out += ["## SASS evidence", "",
-                f"UTCHMMA (tcgen05.mma): {sass.count('UTCHMMA')}  ·  UTMALDG (TMA load): {sass.count('UTMALDG')}  ·  "
-                f"LDTM (tcgen05.ld): {sass.count('LDTM')}  ·  UTCBAR (tcgen05.commit): {sass.count('UTCBAR')}", "",
+                f"HGMMA (wgmma): {sass.count('HGMMA')}  ·  UTMALDG (TMA load): {sass.count('UTMALDG')}  ·  "
+                f"WARPGROUP.DEPBAR (wgmma.wait_group): {sass.count('WARPGROUP.DEPBAR')}  ·  SYNCS (mbarrier): {sass.count('SYNCS')}", "",
                 "## top warp-stall sampling sites (first captured launch)", "", "| samples | share | SASS |", "|---:|---:|---|"]
         for n, s in sorted(rows, reverse=True)[:15]:
             out.append(f"| {n} | {100 * n / tot:.1f}% | `{s[:90]}` |")

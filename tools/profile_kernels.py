@@ -2,11 +2,12 @@
 
     python tools/profile_kernels.py [--precision tf32|bf16] [--only NAME] [--iters 20] [--out gpurun_out/kernels.json]
 
-``--precision tf32`` (default, the engine's default): fp32 tensors, tcgen05 kind::tf32 convolutions (compute roofline =
-half of the measured bf16 tensor throughput), fp32 CUDA-core Linear with the SGD update fused into the weight-gradient pass.
+``--precision tf32`` (default, the engine's default): fp32 tensors, wgmma tf32 convolutions (compute roofline =
+half of the bf16 tensor throughput), fp32 CUDA-core Linear with the SGD update fused into the weight-gradient pass.
 
-Roofline denominators: MEASURED_PEAKS.json (hbm_gbs, bf16_tflops burst).  For the fused cut kernels the target time is
-max(FLOPs / peak, link bytes / 770 GB/s) as the profiling recipe prescribes.  Under ``ncu`` use ``--only`` + ``--iters 1``.
+Roofline denominators: MEASURED_PEAKS.json (hbm_gbs, bf16_tflops) when present, else the H100 SXM data sheet (3.35 TB/s HBM3,
+989 TFLOP/s dense bf16 at 700 W; a card with a lower power limit reaches less).  For the fused cut kernels the target time
+is max(FLOPs / peak, link bytes / NVLINK_GBS).  Under ``ncu`` use ``--only`` + ``--iters 1``.
 """
 import argparse
 import json
@@ -19,12 +20,12 @@ import torch
 
 from split_learning_b200.ops import native as N
 
-PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "src": "fallback"}
+PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "src": "H100 SXM data sheet"}
 pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
 if os.path.exists(pk):
     d = json.load(open(pk))
     PEAKS = {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "src": "measured"}
-NVLINK_GBS = 770.0
+NVLINK_GBS = 450.0                  # NVLink 4, one direction (data sheet)
 
 _flush = None
 
@@ -293,7 +294,7 @@ def main():
     global PREC
     PREC = a.precision
     res = {"peaks": PEAKS, "precision": PREC, "gpu": torch.cuda.get_device_name(0), "kernels": {}}
-    fp32_cuda_tflops = 148 * 128 * 2 * 1.965e9 / 1e12          # FFMA peak of the CUDA cores (148 SMs x 128 lanes, 1965 MHz)
+    fp32_cuda_tflops = N.num_sms() * 128 * 2 * 1.98e9 / 1e12   # FFMA peak of the CUDA cores (SMs x 128 lanes, 1980 MHz max clock)
     for name, fn in CASES.items():
         if a.only and a.only != name:
             continue

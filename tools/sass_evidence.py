@@ -1,7 +1,7 @@
-"""SASS/PTX evidence that the kernels are Blackwell-native (B200_PROFILING.md table): counts of UTCHMMA (tcgen05.mma),
-UTMALDG (TMA), LDTM (tcgen05.ld), UTCBAR (tcgen05.commit), REDG/RED vector reductions, per kernel of ops/_slb200.so.
+"""SASS/PTX evidence that the kernels are Hopper-native: counts of HGMMA (wgmma.mma_async), WARPGROUP (wgmma fences /
+wait_group), UTMALDG (TMA), SYNCS (mbarrier), REDG/RED vector reductions, per kernel of ops/_slb200.so.
 
-    python tools/sass_evidence.py > profiles/sass_evidence.md      (runs on the CPU box: cuobjdump only)
+    python tools/sass_evidence.py > profiles/sass_evidence.md      (no GPU needed: cuobjdump only)
 """
 import collections
 import os
@@ -11,7 +11,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "split_learning_b200", "ops", "_slb200.so")
-MN = ["UTCHMMA", "UTMALDG", "LDTM", "UTCBAR", "UTCATOM", "SYNCS", "RED", "HMMA", "LDGSTS", "ST.E", "MEMBAR"]
+MN = ["HGMMA", "WARPGROUP", "UTMALDG", "SYNCS", "RED", "HMMA", "LDGSTS", "ST.E", "MEMBAR"]
 
 
 def main():
@@ -29,14 +29,14 @@ def main():
         for k in MN:
             if re.search(r"\b" + re.escape(k), line):
                 counts[cur][k] += 1
-    print("# SASS evidence (cuobjdump -sass split_learning_b200/ops/_slb200.so, sm_100a)\n")
-    print("`UTCHMMA` = tcgen05.mma, `UTMALDG` = cp.async.bulk.tensor (TMA), `LDTM` = tcgen05.ld, `UTCBAR` = tcgen05.commit;"
-          " no legacy `HMMA` (mma.sync/wmma) anywhere.\n")
+    print("# SASS evidence (cuobjdump -sass split_learning_b200/ops/_slb200.so, sm_90a)\n")
+    print("`HGMMA` = wgmma.mma_async, `WARPGROUP` = wgmma.fence / wait_group, `UTMALDG` = cp.async.bulk.tensor (TMA),"
+          " `SYNCS` = mbarrier; no legacy `HMMA` (mma.sync/wmma) anywhere.\n")
     print("| kernel | " + " | ".join(MN) + " |\n|---|" + "---:|" * len(MN))
     for k, c in counts.items():
         print(f"| `{k[:70]}` | " + " | ".join(str(c.get(m, 0)) for m in MN) + " |")
     ptx = subprocess.run(["cuobjdump", "-ptx", LIB], capture_output=True, text=True).stdout
-    for pat in ("tcgen05.mma", "tcgen05.ld", "tcgen05.alloc", "tcgen05.commit", "cp.async.bulk.tensor", "griddepcontrol", "red.global.add.v4.f32",
+    for pat in ("wgmma.mma_async", "wgmma.wait_group", "mbarrier.try_wait", "cp.async.bulk.tensor", "griddepcontrol", "red.global.add.v4.f32",
                 "st.release.sys", "ld.acquire.sys"):
         print(f"\n* PTX `{pat}`: {ptx.count(pat)} occurrences" if ptx else "", end="")
     print()

@@ -1,8 +1,9 @@
 """Committed SASS listings (BASELINE.json: "each shown in a committed SASS listing"): for every named hot kernel, the
-instructions around its tensor-core mainloop (UTCHMMA = tcgen05.mma, UTMALDG = TMA, UTCBAR = tcgen05.commit) and its
-epilogue (LDTM = tcgen05.ld, peer ST / RED / ST.E.STRONG.SYS stores) cut out of ``cuobjdump -sass`` of the in-tree library.
+instructions around its tensor-core mainloop (HGMMA = wgmma.mma_async, WARPGROUP = wgmma fences / wait_group, UTMALDG =
+TMA, SYNCS = mbarrier) and its epilogue (peer ST / RED / ST.E.STRONG.SYS stores) cut out of ``cuobjdump -sass`` of the
+in-tree library.
 
-    python tools/sass_listings.py          # writes profiles/sass/*.sass + profiles/sass/README.md   (CPU box: cuobjdump only)
+    python tools/sass_listings.py          # writes profiles/sass/*.sass + profiles/sass/README.md   (no GPU needed: cuobjdump only)
 """
 import os
 import re
@@ -22,14 +23,14 @@ KERNELS = {
     "sgd_momentum": "_ZN3slb19sgd_momentum_kernelEP6float4S1_S1_P5uint2xffi",
     "attn_fwd": "_ZN3slb15attn_fwd_kernelE14CUtensorMap_stS0_S0_NS_10AttnParamsE",
     "attn_bwd": "_ZN3slb15attn_bwd_kernelE14CUtensorMap_stS0_S0_S0_NS_10AttnParamsE",
-    "linear_fwd_f32_ffma2_ldgsts": "_ZN3slb21linear_fwd_f32_kernelEPKfS1_Pfiiiiiii",
-    "linear_dgrad_f32_ffma2_ldgsts": "_ZN3slb23linear_dgrad_f32_kernelEPKfS1_Pfiiiiiii",
+    "linear_fwd_f32_ldgsts": "_ZN3slb21linear_fwd_f32_kernelEPKfS1_Pfiiiiiii",
+    "linear_dgrad_f32_ldgsts": "_ZN3slb23linear_dgrad_f32_kernelEPKfS1_Pfiiiiiii",
     "ticket_publish": "_ZN3slb21ticket_publish_kernelEPjijjPKjj",
     "ticket_claim": "_ZN3slb19ticket_claim_kernelEPjijyPVj",
     "zero_wait_flag_acquire": "_ZN3slb16zero_wait_kernelEP6float4xPKjPjyPi",
     "litmus_pingpong": "_ZN3slb22litmus_pingpong_kernelEPjS0_PKjS2_ijiyS0_",
 }
-MARK = re.compile(r"UTC[A-Z]*MMA|UTMALDG|UTCBAR|LDTM|UTCATOMSWS|RED\.|REDG|ST\.E\.STRONG\.SYS|LD\.E\.STRONG\.SYS|SYNCS|MEMBAR|ACQBULK|UTMAPF|ERRBAR|CCTL|FFMA2|LDGSTS|ATOM")
+MARK = re.compile(r"HGMMA|WARPGROUP|UTMALDG|RED\.|REDG|ST\.E\.STRONG\.SYS|LD\.E\.STRONG\.SYS|SYNCS|MEMBAR|UTMAPF|ERRBAR|CCTL|LDGSTS|ATOM")
 
 
 def listing(mangled):
@@ -41,10 +42,10 @@ def listing(mangled):
 
 def main():
     os.makedirs(DST, exist_ok=True)
-    readme = ["# SASS listings of the named hot kernels (sm_100a, `cuobjdump -sass split_learning_b200/ops/_slb200.so`)", "",
-              "Each file holds the instruction windows around the tensor-core / TMA / TMEM / peer-memory instructions of one kernel "
+    readme = ["# SASS listings of the named hot kernels (sm_90a, `cuobjdump -sass split_learning_b200/ops/_slb200.so`)", "",
+              "Each file holds the instruction windows around the tensor-core / TMA / mbarrier / peer-memory instructions of one kernel "
               "(full functions are thousands of lines; `tools/sass_listings.py` regenerates these from the in-tree library).", "",
-              "| kernel | file | instructions | UTC*MMA | UTMALDG | LDTM | UTCBAR | RED | sys-scope ld/st | HMMA |", "|---|---|---:|---:|---:|---:|---:|---:|---:|---:|"]
+              "| kernel | file | instructions | HGMMA | UTMALDG | WARPGROUP | SYNCS | RED | sys-scope ld/st | HMMA |", "|---|---|---:|---:|---:|---:|---:|---:|---:|---:|"]
     for name, mangled in KERNELS.items():
         lines = listing(mangled)
         if not lines:
@@ -61,12 +62,12 @@ def main():
             prev = i
         demangled = subprocess.run(["c++filt", mangled], capture_output=True, text=True).stdout.strip()
         with open(os.path.join(DST, name + ".sass"), "w") as f:
-            f.write(f"// {demangled}\n// {len(lines)} instructions; windows around tcgen05 / TMA / TMEM / reduction / system-scope instructions\n")
+            f.write(f"// {demangled}\n// {len(lines)} instructions; windows around wgmma / TMA / mbarrier / reduction / system-scope instructions\n")
             f.write("\n".join(out[:1200]) + "\n")
         txt = "\n".join(lines)
         c = lambda p: len(re.findall(p, txt))
-        readme.append(f"| `{demangled[:90]}` | `{name}.sass` | {len(lines)} | {c(r'UTC[A-Z]*MMA')} | {c('UTMALDG')} | {c('LDTM')} | {c('UTCBAR')} | "
-                      f"{c(r'RED[G.]')} | {c(r'STRONG.SYS')} | {c('HMMA') - c('UTCHMMA')} |")
+        readme.append(f"| `{demangled[:90]}` | `{name}.sass` | {len(lines)} | {c('HGMMA')} | {c('UTMALDG')} | {c('WARPGROUP')} | {c('SYNCS')} | "
+                      f"{c(r'RED[G.]')} | {c(r'STRONG.SYS')} | {c(r'\bHMMA')} |")
     open(os.path.join(DST, "README.md"), "w").write("\n".join(readme) + "\n")
     print("\n".join(readme))
 

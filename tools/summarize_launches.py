@@ -1,6 +1,6 @@
 """ncu launch list (``--metrics gpu__time_duration.sum --csv``) → per-kernel markdown table.
 
-    python tools/summarize_launches.py gpurun_out/launches.csv profiles/launches_r1.md "title"
+    python tools/summarize_launches.py launches.csv profiles/launches.md "title"
 """
 import collections
 import csv

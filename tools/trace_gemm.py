@@ -1,8 +1,8 @@
-"""Cycle stamps of CTA (0,0,0) of the conv kernels: where does one launch spend its time?  (clock64 at 1.965 GHz)
+"""Cycle stamps of CTA (0,0,0) of the conv kernels: where does one launch spend its time?  (clock64 cycles at GHZ)
 
     python tools/trace_gemm.py [tf32|bf16]
-stamps: 0 entry | 1 setup done (barriers, TMEM alloc) | 2 griddepcontrol.wait returned | 3 producer: ring of loads issued
-        4 first operands landed | 5 last operands landed | 6 accumulator complete | 7 TMEM drained, stores/reds issued
+stamps: 0 entry | 1 setup done (barriers) | 2 griddepcontrol.wait returned | 3 producer: ring of loads issued
+        4, 5 unused | 6 accumulator complete | 7 accumulators drained, stores/reds issued
         8 reds visible (split-K) | 9 epilogue done | 10 CTA exit
 """
 import ctypes
@@ -15,7 +15,7 @@ import torch
 
 from split_learning_b200.ops import native as N
 
-GHZ = 1.965
+GHZ = 1.98                       # H100 maximum SM clock (a power-capped card may run lower)
 
 
 def main():

@@ -85,7 +85,7 @@ def main():
                     if ks > max(1, k_iters // 2):
                         continue
                     tiles = ((M + 127) // 128) * (Nn // bn) * ks
-                    if tiles > 148 * 4:
+                    if tiles > N.num_sms() * 4:
                         continue
                     if not flip:
                         fn = lambda: N.conv3x3_fwd(x, w, out, bias, s1, s2, acc=acc, tiling=(bn, ks), counters=ctr)
@@ -105,7 +105,7 @@ def main():
                 continue
             m_tiles = (9 * Cout + 127) // 128
             for ks in (1, 2, 3, 4, 6, 8, 12, 16, 24, 32):
-                if ks > max(1, k_iters // 2) or m_tiles * (Cin // bn) * ks > 148 * 4:
+                if ks > max(1, k_iters // 2) or m_tiles * (Cin // bn) * ks > N.num_sms() * 4:
                     continue
                 t = timeit(lambda: N.conv3x3_wgrad(x, dy, dw, k_split=ks, block_n=bn), a.iters)
                 if best is None or t < best[0]:
