@@ -143,7 +143,8 @@ class SequentialServer(Server):
             ok = True
             if self.validation and full:
                 from ..validation import get_val
-                ok, val = get_val(self.model_name, self.data_name, full, self.logger, strict=self.STRICT_VALIDATION)
+                ok, val = get_val(self.model_name, self.data_name, full, self.logger, strict=self.STRICT_VALIDATION,
+                                  native=self.cfg.b200.get("native-validation", False))
                 metrics.update(val)
             if ok:
                 if full and self.save_parameters:
@@ -335,7 +336,8 @@ class FlexServer(Server):
                 ok = True
                 if self.validation and full:
                     from ..validation import get_val
-                    ok, val = get_val(self.model_name, self.data_name, full, self.logger)
+                    ok, val = get_val(self.model_name, self.data_name, full, self.logger,
+                                      native=self.cfg.b200.get("native-validation", False))
                     metrics.update(val)
                 if ok and full:
                     save_checkpoint(full, checkpoint_path(self.model_name, self.data_name, self.workdir))
@@ -481,7 +483,8 @@ class TwoLSServer(Server):
             ok = True
             if self.validation:
                 from ..validation import get_val
-                ok, val = get_val(self.model_name, self.data_name, self.global_model, self.logger)
+                ok, val = get_val(self.model_name, self.data_name, self.global_model, self.logger,
+                                  native=self.cfg.b200.get("native-validation", False))
                 metrics.update(val)
             self.round = self.round - 1 if ok else 0
         else:

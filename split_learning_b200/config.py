@@ -37,6 +37,7 @@ DEFAULT_B200 = {
     "synthetic-data": False,
     "routing": "round-robin",      # competing-consumer emulation on the device plane
     "data-plane": "host",          # host = broker queues (any device) | device = peer-memory mailboxes (CUDA)
+    "native-validation": False,    # false = torch modules | true = native eval plan (error if unsupported) | auto
 }
 
 

@@ -64,6 +64,22 @@ class GpuImageLoader:
             yield self.batch(order[k * self.batch_size:(k + 1) * self.batch_size])
 
 
+class ResidentBatches:
+    """Iterable of (x, y) slices of device-resident tensors, in order, ``batch_size`` at a time (short batch last)."""
+
+    def __init__(self, x: torch.Tensor, y: torch.Tensor, batch_size: int, device):
+        self.x = x.to(device).contiguous()
+        self.y = y.long().to(device)
+        self.batch_size = int(batch_size)
+
+    def __len__(self):
+        return (self.x.shape[0] + self.batch_size - 1) // self.batch_size
+
+    def __iter__(self):
+        for lo in range(0, self.x.shape[0], self.batch_size):
+            yield self.x[lo:lo + self.batch_size], self.y[lo:lo + self.batch_size]
+
+
 def reference_batch(images_u8, idx, dx, dy, flip, mean, std, pad: int = 4):
     """The same transform with plain torch ops (numerics oracle of the kernel)."""
     x = images_u8[idx].permute(0, 3, 1, 2).float() / 255.0

@@ -220,6 +220,31 @@ def gpu_image_loader(name: str, batch_size: int, distribution: Sequence[int], de
 _WARNED: set = set()
 
 
+def _synthetic_default(name: str, root: str) -> bool:
+    return os.environ.get("SLB200_SYNTHETIC", "0") == "1" or not real_data_available(name, root)
+
+
+def resident_test_loader(data_name: str, device, synthetic: Optional[bool] = None, root: str = "./data", seed: int = 0):
+    """The test split of ``data_loader(data_name, train=False)`` held in HBM: the same samples in the same order and batches
+    (100, short batch last), so results compare sample for sample.  Real CIFAR10: the uint8 [10000, 32, 32, 3] split is
+    uploaded once and each batch is one ``image_batch`` launch with crop and flip off (= ToTensor + Normalize).  Synthetic:
+    the same ``SyntheticDataset`` test samples, resident as fp32."""
+    from .gpu_loader import CIFAR_MEAN, CIFAR_STD, GpuImageLoader, ResidentBatches
+    name = str(data_name).upper()
+    if name != "CIFAR10":
+        raise ValueError(f"no resident test split for {data_name}")
+    if synthetic is None:
+        synthetic = _synthetic_default(name, root)
+    shape, _, ncls, test_bs = DATASET_SHAPES[name]
+    if synthetic:
+        ds = SyntheticDataset(name, [max(1, 100 // ncls)] * ncls, seed=seed + 7919)
+        return ResidentBatches(ds.data, ds.labels, test_bs, device)
+    import torchvision
+    ds = torchvision.datasets.CIFAR10(root=root, train=False, download=False)
+    return GpuImageLoader(torch.from_numpy(ds.data), torch.tensor(ds.targets), test_bs, device, CIFAR_MEAN, CIFAR_STD,
+                          augment=False, shuffle=False)
+
+
 def data_loader(data_name: Optional[str] = None, batch_size: Optional[int] = None,
                 distribution: Optional[Sequence[int]] = None, train: bool = True,
                 synthetic: Optional[bool] = None, root: str = "./data", seed: int = 0, device=None,
@@ -229,7 +254,7 @@ def data_loader(data_name: Optional[str] = None, batch_size: Optional[int] = Non
         raise ValueError(f"Dataset {data_name} not supported.")
     explicit = synthetic is not None or os.environ.get("SLB200_SYNTHETIC", "0") == "1"
     if synthetic is None:
-        synthetic = os.environ.get("SLB200_SYNTHETIC", "0") == "1" or not real_data_available(name, root)
+        synthetic = _synthetic_default(name, root)
     if synthetic and not explicit and name not in _WARNED:
         # never train on noise silently: the reference would download the dataset or fail (src/dataset/dataloader.py:61-84)
         _WARNED.add(name)

@@ -5,6 +5,7 @@
 // pointers, and the mailbox flag primitives.  All vectorised to 16-byte accesses.
 #include "sm90.cuh"
 
+#include <climits>
 #include <map>
 #include <mutex>
 #include <utility>
@@ -234,7 +235,9 @@ struct BnFwdParams {
   uint32_t* hint;
 };
 
-template <typename T>
+// INFER: BatchNorm in inference mode (module.eval()): scale / shift from running_mean / running_var, no batch statistics
+// and no writes to the running statistics, num_batches_tracked or save_*.
+template <typename T, bool INFER = false>
 __global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const BnFwdParams<T> p) {
   pdl_trigger();
   pdl_wait();
@@ -243,6 +246,13 @@ __global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const BnFwdParams
   float* s_shift = s_aff + p.C;
   const float invP = 1.f / static_cast<float>(p.P);
   for (int c = threadIdx.x; c < p.C; c += blockDim.x) {
+    if constexpr (INFER) {
+      const float invstd = rsqrtf(p.running_var[c] + p.eps);
+      const float g = p.gamma[c];
+      s_scale[c] = g * invstd;
+      s_shift[c] = p.beta[c] - p.running_mean[c] * g * invstd;
+      continue;
+    }
     if (p.identity) { s_scale[c] = 1.f; s_shift[c] = 0.f; continue; }
     const float mean = p.sum[c] * invP;
     const float var = fmaxf(p.sumsq[c] * invP - mean * mean, 0.f);
@@ -260,7 +270,8 @@ __global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const BnFwdParams
       }
     }
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0 && p.update_running && !p.identity && p.num_batches_tracked) *p.num_batches_tracked += 1;
+  if (!INFER && blockIdx.x == 0 && threadIdx.x == 0 && p.update_running && !p.identity && p.num_batches_tracked)
+    *p.num_batches_tracked += 1;
   __syncthreads();
 
   const int cg = p.C >> 3;                                  // 8-channel groups
@@ -1346,6 +1357,63 @@ __global__ void ce_fwd_bwd_kernel(const float* logits, const long long* labels, 
   }
 }
 
+// ============================================================================ evaluation loss / accuracy
+// (value, index) of a row maximum with torch.argmax's rules: a NaN beats every number, and among equal values (or NaNs)
+// the smaller index wins.  idx == INT_MAX marks "no element yet".
+__device__ __forceinline__ bool argmax_better(float v, int i, float best, int bi) {
+  if (bi == INT_MAX) return true;
+  const bool vn = v != v, bn = best != best;
+  if (vn || bn) return vn && (!bn || i < bi);
+  return v > best || (v == best && i < bi);
+}
+
+// One block of 8 warps, warp w takes rows w, w + 8, ...: per row the max-subtracted log-sum-exp (fp64) and the argmax.
+// The batch-mean loss is added to loss_total (fp64), the correct predictions to correct and B to count.  Every sum runs
+// in a fixed order, so the totals are the same bits every run.  Nothing that changes per batch is a launch argument.
+__global__ void __launch_bounds__(256) eval_metrics_kernel(const float* logits, const long long* labels, int B, int C,
+                                                           double* loss_total, long long* correct, long long* count) {
+  pdl_trigger();
+  pdl_wait();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  __shared__ double s_loss[32];
+  __shared__ long long s_hit[32];
+  double wl = 0.0;
+  long long wh = 0;
+  for (int r = warp; r < B; r += nw) {
+    const float* row = logits + (long long)r * C;
+    float best = 0.f;
+    int bi = INT_MAX;
+    for (int c = lane; c < C; c += 32) {
+      const float v = row[c];
+      if (argmax_better(v, c, best, bi)) { best = v; bi = c; }
+    }
+    for (int o = 16; o; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (oi != INT_MAX && argmax_better(ov, oi, best, bi)) { best = ov; bi = oi; }
+    }
+    const double mx = static_cast<double>(best);
+    double se = 0.0;
+    for (int c = lane; c < C; c += 32) se += exp(static_cast<double>(row[c]) - mx);
+    for (int o = 16; o; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+    if (lane == 0) {
+      const long long lab = labels[r];
+      wl += mx + log(se) - static_cast<double>(row[lab]);
+      wh += (bi == lab) ? 1 : 0;
+    }
+  }
+  if (lane == 0) { s_loss[warp] = wl; s_hit[warp] = wh; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    long long h = 0;
+    for (int w = 0; w < nw; ++w) { s += s_loss[w]; h += s_hit[w]; }
+    *loss_total += s / static_cast<double>(B);
+    *correct += h;
+    *count += B;
+  }
+}
+
 // ============================================================================ optimisers (flat)
 // v = mu*v + g ; p -= lr*v ; g = 0 ; optional bf16 shadow copy of p  (torch.optim.SGD, no dampening/nesterov/wd)
 __global__ void sgd_momentum_kernel(float4* p, float4* g, float4* m, uint2* p_bf16, long long n4, float lr, float mu, int first_step) {
@@ -1483,7 +1551,7 @@ int slb_preload_elementwise() {
   bad += slb_det(nullptr).part != nullptr ? 0 : 1;                // reduction scratch, before any graph capture
 #define SLB_PRELOAD(k) bad += (cudaFuncGetAttributes(&a, k) != cudaSuccess)
 #define SLB_PRELOAD_T(T) \
-  { auto k = bn_relu_pool_fwd_kernel<T>; SLB_PRELOAD(k); } \
+  { auto k = bn_relu_pool_fwd_kernel<T>; SLB_PRELOAD(k); } { auto k = bn_relu_pool_fwd_kernel<T, true>; SLB_PRELOAD(k); } \
   { auto k = bn_bwd_reduce_kernel<true, T>; SLB_PRELOAD(k); } { auto k = bn_bwd_reduce_kernel<false, T>; SLB_PRELOAD(k); } \
   { auto k = bn_bwd_apply_kernel<true, T>; SLB_PRELOAD(k); } { auto k = bn_bwd_apply_kernel<false, T>; SLB_PRELOAD(k); } \
   { auto k = bn_bwd_fused_kernel<true, T>; SLB_PRELOAD(k); } { auto k = bn_bwd_fused_kernel<false, T>; SLB_PRELOAD(k); } \
@@ -1499,7 +1567,7 @@ int slb_preload_elementwise() {
   SLB_PRELOAD(zero_kernel); SLB_PRELOAD(zero_wait_kernel); SLB_PRELOAD(wait_flag_kernel); SLB_PRELOAD(set_flag_kernel); SLB_PRELOAD(counter_inc_kernel);
   SLB_PRELOAD(linear_fwd_f32_kernel); SLB_PRELOAD(linear_dgrad_f32_kernel); SLB_PRELOAD(linear_wgrad_f32_kernel);
   SLB_PRELOAD(sumsq_kernel); SLB_PRELOAD(clip_scale_kernel);
-  SLB_PRELOAD(ce_fwd_bwd_kernel); SLB_PRELOAD(sgd_momentum_kernel); SLB_PRELOAD(adamw_kernel); SLB_PRELOAD(cast_f32_bf16_kernel);
+  SLB_PRELOAD(ce_fwd_bwd_kernel); SLB_PRELOAD(eval_metrics_kernel); SLB_PRELOAD(sgd_momentum_kernel); SLB_PRELOAD(adamw_kernel); SLB_PRELOAD(cast_f32_bf16_kernel);
   SLB_PRELOAD(fedavg_kernel); SLB_PRELOAD(image_batch_kernel);
 #undef SLB_PRELOAD_T
 #undef SLB_PRELOAD
@@ -1569,6 +1637,27 @@ int slb_bn_relu_pool_fwd(const void* y, const float* sum, const float* sumsq, co
                            relu, pool, momentum, eps, update_running, identity, ticket, flag, seq, hint, st);
   return bn_fwd_t<__nv_bfloat16>(y, sum, sumsq, gamma, beta, running_mean, running_var, nbt, save_mean, save_invstd, out, P, C,
                                  H, W, relu, pool, momentum, eps, update_running, identity, ticket, flag, seq, hint, st);
+}
+
+}  // extern "C"
+template <typename T>
+static int bn_infer_t(const void* y, const float* gamma, const float* beta, const float* running_mean, const float* running_var,
+                      void* out, int P, int C, int H, int W, int relu, int pool, float eps, cudaStream_t st) {
+  BnFwdParams<T> p = {reinterpret_cast<const T*>(y), nullptr, nullptr, gamma, beta, const_cast<float*>(running_mean),
+                      const_cast<float*>(running_var), nullptr, nullptr, nullptr, reinterpret_cast<T*>(out), P, C, H, W, relu,
+                      pool, 0.f, eps, 0, 0, nullptr, nullptr, nullptr, nullptr};
+  const long long work = (pool ? (long long)P / 4 : P) * (C / 8);
+  launch_k(bn_relu_pool_fwd_kernel<T, true>, grid_for(work, 256, 132 * 4), 256, 2 * C * sizeof(float), st, p);
+  return last_err();
+}
+extern "C" {
+// BatchNorm (inference mode) + ReLU + MaxPool2 forward: the running statistics are read, never written.
+int slb_bn_relu_pool_infer(const void* y, const float* gamma, const float* beta, const float* running_mean,
+                           const float* running_var, void* out, int P, int C, int H, int W, int relu, int pool, float eps,
+                           int dtype, cudaStream_t st) {
+  if (C % 8 || gamma == nullptr || beta == nullptr || running_mean == nullptr || running_var == nullptr) return -1;
+  if (dtype == 1) return bn_infer_t<float>(y, gamma, beta, running_mean, running_var, out, P, C, H, W, relu, pool, eps, st);
+  return bn_infer_t<__nv_bfloat16>(y, gamma, beta, running_mean, running_var, out, P, C, H, W, relu, pool, eps, st);
 }
 
 }  // extern "C"
@@ -1819,6 +1908,12 @@ int slb_ce_fwd_bwd(const float* logits, const long long* labels, float* dlogits,
   const Det det = slb_det(st);
   if (det.part == nullptr) return -30;
   launch_k(ce_fwd_bwd_kernel, (B * 32 + 127) / 128, 128, 0, st, logits, labels, dlogits, loss_sum, nan_flag, B, C, ldd, det);
+  return last_err();
+}
+int slb_eval_metrics(const float* logits, const long long* labels, int B, int C, double* loss_total, long long* correct,
+                     long long* count, cudaStream_t st) {
+  if (B < 1 || C < 1) return -1;
+  launch_k(eval_metrics_kernel, 1, 256, 0, st, logits, labels, B, C, loss_total, correct, count);
   return last_err();
 }
 int slb_sgd_momentum(float* p, float* g, float* m, void* p_bf16, long long n, float lr, float mu, int first_step, cudaStream_t st) {

@@ -300,6 +300,15 @@ def bn_relu_pool_fwd(y, col_sum, col_sumsq, gamma, beta, running_mean, running_v
                                       _dt(y), _stream()), "bn_relu_pool_fwd")
 
 
+def bn_relu_pool_infer(y, gamma, beta, running_mean, running_var, out, H, W, relu, pool, eps=1e-5):
+    """BatchNorm in inference mode (``invstd = rsqrt(running_var + eps)``) + ReLU + MaxPool2 on NHWC ``y``; reads the
+    running statistics and writes nothing but ``out``."""
+    P, C = y.shape[0] * y.shape[1] * y.shape[2], y.shape[3]
+    _check(lib().slb_bn_relu_pool_infer(_p(y), _p(gamma), _p(beta), _p(running_mean), _p(running_var), _p(out), c_int(P),
+                                        c_int(C), c_int(H), c_int(W), c_int(int(relu)), c_int(int(pool)), c_float(eps), _dt(y),
+                                        _stream()), "bn_relu_pool_infer")
+
+
 BN_BWD_CHAN_MAX_P = int(os.environ.get("SLB200_BN_BWD_CHAN_MAX_P", "4096"))
 
 
@@ -409,6 +418,16 @@ def ce_fwd_bwd(logits_f32, labels_i64, dlogits_f32, loss_sum, nan_flag):
     B, C = logits_f32.shape
     _check(lib().slb_ce_fwd_bwd(_p(logits_f32), _p(labels_i64), _p(dlogits_f32), _p(loss_sum), _p(nan_flag), c_int(B),
                                 c_int(C), c_int(dlogits_f32.stride(0)), _stream()), "ce_fwd_bwd")
+
+
+def eval_metrics(logits_f32, labels_i64, loss_total_f64, correct_i64, count_i64):
+    """Evaluation totals of one batch: loss_total += mean cross-entropy (fp64), correct += #(argmax == label) (torch.argmax
+    rules: first maximum, NaN counts as the maximum), count += B.  Fixed summation order: bit-reproducible."""
+    B, C = logits_f32.shape
+    if logits_f32.stride(1) != 1 or logits_f32.stride(0) != C:
+        raise NativeError("eval_metrics needs contiguous [B, C] logits")
+    _check(lib().slb_eval_metrics(_p(logits_f32), _p(labels_i64), c_int(B), c_int(C), _p(loss_total_f64), _p(correct_i64),
+                                  _p(count_i64), _stream()), "eval_metrics")
 
 
 def sgd_momentum(p, g, m, p_bf16, lr, mu, first_step=False):

@@ -471,7 +471,8 @@ class Server:
             ok = True
             if self.validation and full:
                 from .validation import get_val
-                ok, val = get_val(self.model_name, self.data_name, full, self.logger)
+                ok, val = get_val(self.model_name, self.data_name, full, self.logger,
+                                  native=self.cfg.b200.get("native-validation", False))
                 metrics.update(val)
             if ok:
                 if full:

@@ -13,6 +13,11 @@ over flat fp32 master / gradient / momentum buffers.  Forward, backward(+recompu
 optimizer step of one microbatch are captured once per batch size into CUDA graphs; the host
 only copies the input in and replays.
 
+The same block sequence also runs in eval mode (``eval_forward``, ``train/b200_eval.py``): conv without BN statistics,
+BatchNorm on the running statistics, dropout skipped, always the fp32 (tf32) flavour, forward buffers only, one CUDA
+graph per batch size.  ``eval_only=True`` builds an executor for that alone (no gradient, momentum, bf16 shadow or
+exportable memory).
+
 Two compute precisions (``precision=`` / ``b200.precision`` / ``SLB200_PRECISION``):
 
 * ``tf32`` (default, the reference's precision): fp32 activations and weights end to end,
@@ -206,9 +211,12 @@ def flat_layouts(model_cls, start_layer: int, end_layer: int):
 class B200Executor(StageExecutor):
     def __init__(self, model: SplitModel, model_name: str, learning: dict, device, is_first=False, is_last=False,
                  recompute: bool = True, use_graphs: bool = True, seed: int = 1234, fused_cut: bool = True,
-                 precision: Optional[str] = None):
+                 precision: Optional[str] = None, eval_only: bool = False, state_dict: Optional[Dict[str, torch.Tensor]] = None):
         N.require()
         import os
+        self.eval_only = eval_only
+        if eval_only:
+            precision = "tf32"
         precision = (precision or learning.get("precision") or os.environ.get("SLB200_PRECISION") or "tf32").lower()
         if precision in ("fp32", "float32"):
             precision = "tf32"
@@ -245,8 +253,9 @@ class B200Executor(StageExecutor):
         (self.in_kind, self.in_shape), self.blocks, (self.out_kind, self.out_shape) = compile_plan(model)
         self.num_classes = model.num_classes() if is_last else None
         self._layout_params(model)
-        self.load_state_dict(model.state_dict())
+        self.load_state_dict(state_dict if state_dict is not None else model.state_dict())
         self.plans: Dict[int, "_Plan"] = {}
+        self.eval_plans: Dict[int, "_Plan"] = {}
         self.step_ctr = torch.zeros(1, device=self.device, dtype=torch.int32)
         self.nan_flag = torch.zeros(1, device=self.device, dtype=torch.int32)
         self.loss_buf = torch.zeros(4, device=self.device)       # [0] = mean CE loss of the last microbatch
@@ -301,13 +310,20 @@ class B200Executor(StageExecutor):
                 hi = max(_align(self.entries[k][0] + math.prod(self.entries[k][1])) for k in keys)
                 self.block_range[bi] = (lo, hi)
         dev = self.device
-        # The fp32 master lives in an IPC-exportable allocation: the round-end FedAvg all-reduce (parallel/allreduce.py)
-        # reads and writes the replicas' masters in place over NVLink — no staging copy, no START payload next round.
-        from ..parallel.mailbox import alloc_exportable
-        raw, self.P_handle, _ = alloc_exportable(self.n_params * 4, dev)
-        self.P = raw.view(torch.float32)[:self.n_params]
-        self.G = torch.zeros(self.n_params, device=dev)
-        self.M = torch.zeros(self.n_params, device=dev)
+        if self.eval_only:                               # inference: parameters and statistics only, process-private
+            def alloc(n):
+                return torch.zeros(n, device=dev), None
+        else:
+            # The fp32 master lives in an IPC-exportable allocation: the round-end FedAvg all-reduce (parallel/allreduce.py)
+            # reads and writes the replicas' masters in place over NVLink — no staging copy, no START payload next round.
+            from ..parallel.mailbox import alloc_exportable
+
+            def alloc(n):
+                raw, handle, _ = alloc_exportable(n * 4, dev)
+                return raw.view(torch.float32)[:n], handle
+        self.P, self.P_handle = alloc(self.n_params)
+        self.G = None if self.eval_only else torch.zeros(self.n_params, device=dev)
+        self.M = None if self.eval_only else torch.zeros(self.n_params, device=dev)
         self.PB = None if self.fp32 else torch.zeros(self.n_params, device=dev, dtype=torch.bfloat16)
         # BatchNorm running statistics: one flat exportable buffer S (mean | var per BN, 128-aligned entries) plus a float
         # mirror I of the integer counters (4 floats per BN) that the all-reduce averages-and-rounds (src/Utils.py:59-60)
@@ -323,10 +339,8 @@ class B200Executor(StageExecutor):
                 self.int_entries[f"layer{b.bn}.num_batches_tracked"] = (io, (1,))
                 io += 4
         self.n_stats, self.n_ints = max(so, 128), max(io, 4)
-        raw, self.S_handle, _ = alloc_exportable(self.n_stats * 4, dev)
-        self.S = raw.view(torch.float32)[:self.n_stats]
-        raw, self.I_handle, _ = alloc_exportable(self.n_ints * 4, dev)
-        self.I = raw.view(torch.float32)[:self.n_ints]
+        self.S, self.S_handle = alloc(self.n_stats)
+        self.I, self.I_handle = alloc(self.n_ints)
         self.bn_state: Dict[int, Dict[str, torch.Tensor]] = {}
         for b in self.blocks:
             if isinstance(b, ConvBlock) and b.bn is not None:
@@ -380,21 +394,43 @@ class B200Executor(StageExecutor):
 
     # ------------------------------------------------------------------ plans
     def plan(self, batch: int) -> "_Plan":
+        if self.eval_only:
+            raise RuntimeError("this executor was built with eval_only=True: it has no training plan")
         p = self.plans.get(batch)
         if p is None:
             p = self.plans[batch] = _Plan(self, batch)
         return p
 
+    def eval_plan(self, batch: int) -> "_Plan":
+        p = self.eval_plans.get(batch)
+        if p is None:
+            p = self.eval_plans[batch] = _Plan(self, batch, eval_mode=True)
+        return p
+
+    def eval_forward(self, x: torch.Tensor) -> torch.Tensor:
+        """Eval-mode output of this stage (BatchNorm on running statistics, no dropout, fp32 numerics) in the wire layout of
+        ``forward_only``.  Touches no training state: slots, stored microbatches, step counter, BN statistics, NaN flag."""
+        xi = self._to_internal(x, torch.float32)
+        pl = self.eval_plan(xi.shape[0])
+        self._enter()
+        with torch.cuda.stream(self.stream):
+            pl.x_in[0].copy_(xi, non_blocking=True)
+            pl.run_eval()
+            out = self._from_internal_out(pl.final_out()).clone()
+        self.stream.synchronize()
+        return out
+
     # ------------------------------------------------------------------ StageExecutor API (tensor in / tensor out)
-    def _to_internal(self, x: torch.Tensor) -> torch.Tensor:
+    def _to_internal(self, x: torch.Tensor, dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+        dtype = dtype or self.act_dtype
         x = x.to(self.device, non_blocking=True)
         if self.is_first:
             return x.float().contiguous()
         if self.in_kind == "image":
             if x.dim() == 4 and x.shape[1] == self.in_shape[0] and x.shape[-1] != self.in_shape[0]:
                 x = x.permute(0, 2, 3, 1)                # NCHW wire -> NHWC
-            return x.to(self.act_dtype).contiguous()
-        return x.to(self.act_dtype).contiguous()
+            return x.to(dtype).contiguous()
+        return x.to(dtype).contiguous()
 
     def _from_internal_out(self, t: torch.Tensor) -> torch.Tensor:
         if self.out_kind == "image":
@@ -477,13 +513,18 @@ class B200Executor(StageExecutor):
 
 # ----------------------------------------------------------------------------- per-batch-size plan
 class _Plan:
-    """Static buffers + captured graphs for one batch size."""
+    """Static buffers + captured graphs for one batch size.  ``eval_mode``: the inference forward only (forward buffers,
+    one input slot, fp32 activations and weights whatever the executor's precision)."""
 
-    def __init__(self, ex: B200Executor, B: int):
+    def __init__(self, ex: B200Executor, B: int, eval_mode: bool = False):
         self.ex, self.B = ex, B
+        self.eval = eval_mode
+        train = not eval_mode
+        self.fp32 = ex.fp32 or eval_mode
+        self.ke = 32 if self.fp32 else ex.ke
         dev = ex.device
-        bf = ex.act_dtype                                  # activation dtype of this plan (fp32 in tf32 mode)
-        self.n_slots = ex.slots if (ex.recompute or ex.is_last) else ex.slots
+        bf = torch.float32 if eval_mode else ex.act_dtype  # activation dtype of this plan (fp32 in tf32 mode)
+        self.n_slots = 1 if eval_mode else ex.slots
         self.free = list(range(self.n_slots))
         # ---- stage input slots
         if ex.is_first:
@@ -505,18 +546,19 @@ class _Plan:
             scratch += _align(n, 4)
         for bi, b in enumerate(ex.blocks):
             if isinstance(b, ConvBlock):
-                if b.bn is not None:
+                if b.bn is not None and train:
                     reserve((bi, "sum"), b.cout)
                     reserve((bi, "sumsq"), b.cout)
                 if b.conv is not None and b.cin > 4:
                     M = B * b.H * b.W
-                    if N.conv_tiling(M, b.cout, b.cin, ke=ex.ke)[1] > 1:
+                    if N.conv_tiling(M, b.cout, b.cin, ke=self.ke)[1] > 1:
                         reserve((bi, "facc"), M * b.cout)           # split-K partial sums, forward
-                    if N.conv_tiling(M, b.cin, b.cout, flip=1, ke=ex.ke)[1] > 1 and not (bi == 0 and ex.is_first):
+                    if train and N.conv_tiling(M, b.cin, b.cout, flip=1, ke=ex.ke)[1] > 1 and not (bi == 0 and ex.is_first):
                         reserve((bi, "dacc"), M * b.cin)            # split-K partial sums, dgrad
             elif isinstance(b, LinearBlock):
                 reserve((bi, "acc"), B * b.fout)
-                reserve((bi, "dacc_in"), B * b.fin)
+                if train:
+                    reserve((bi, "dacc_in"), B * b.fin)
         self.scratch = torch.zeros(max(scratch, 4), device=dev)
         # ---- activations
         self.act: List[Dict[str, torch.Tensor]] = []
@@ -526,37 +568,45 @@ class _Plan:
                 OH, OW = (b.H // 2, b.W // 2) if b.pool else (b.H, b.W)
                 if b.conv is not None:
                     d["y"] = torch.zeros(B, b.H, b.W, b.cout, device=dev, dtype=bf)
-                    d["dy"] = torch.zeros(B, b.H, b.W, b.cout, device=dev, dtype=bf)
+                    if train:
+                        d["dy"] = torch.zeros(B, b.H, b.W, b.cout, device=dev, dtype=bf)
                 d["out"] = d["y"] if (b.conv is not None and b.bn is None) else torch.zeros(B, OH, OW, b.cout, device=dev, dtype=bf)
-                d["bwd_bar"] = torch.zeros(4, device=dev, dtype=torch.int32)     # grid-barrier words of the fused BN backward
-                d["save_mean"] = torch.zeros(b.cout, device=dev)
-                d["save_invstd"] = torch.ones(b.cout, device=dev)
-                d["dx"] = torch.zeros(B, b.H, b.W, b.cin, device=dev, dtype=bf) if (b.cin > 4 and b.conv is not None) else None
-                if b.conv is None:
-                    d["dx_orphan"] = torch.zeros(B, b.H, b.W, b.cout, device=dev, dtype=bf)
-                d["dout_bf16"] = torch.zeros(B, OH, OW, b.cout, device=dev, dtype=bf)
+                if train:
+                    d["bwd_bar"] = torch.zeros(4, device=dev, dtype=torch.int32)     # grid-barrier words of the fused BN backward
+                    d["save_mean"] = torch.zeros(b.cout, device=dev)
+                    d["save_invstd"] = torch.ones(b.cout, device=dev)
+                    d["dx"] = torch.zeros(B, b.H, b.W, b.cin, device=dev, dtype=bf) if (b.cin > 4 and b.conv is not None) else None
+                    if b.conv is None:
+                        d["dx_orphan"] = torch.zeros(B, b.H, b.W, b.cout, device=dev, dtype=bf)
+                    d["dout_bf16"] = torch.zeros(B, OH, OW, b.cout, device=dev, dtype=bf)
             elif isinstance(b, DropoutOp):
-                d["out"] = torch.zeros(B, b.n, device=dev, dtype=bf)
-                d["mask"] = torch.zeros(B, b.n, device=dev, dtype=torch.uint8)
-                d["dx"] = torch.zeros(B, b.n, device=dev, dtype=bf)
+                if train:
+                    d["out"] = torch.zeros(B, b.n, device=dev, dtype=bf)
+                    d["mask"] = torch.zeros(B, b.n, device=dev, dtype=torch.uint8)
+                    d["dx"] = torch.zeros(B, b.n, device=dev, dtype=bf)
             else:
                 ld = _align(b.fout, 16)
-                d["out"] = torch.zeros(B, ld, device=dev, dtype=bf)[:, :b.fout]
-                d["dz"] = torch.zeros(B, ld, device=dev, dtype=bf)[:, :b.fout]
-                d["mask"] = torch.zeros(B, b.fout, device=dev, dtype=torch.uint8) if b.drop > 0 else None
-                d["logits"] = torch.zeros(B, b.fout, device=dev) if (bi == len(ex.blocks) - 1 and ex.is_last) else None
-                d["dx_bf16"] = torch.zeros(B, b.fin, device=dev, dtype=bf)
+                final_logits = bi == len(ex.blocks) - 1 and ex.is_last
+                d["logits"] = torch.zeros(B, b.fout, device=dev) if final_logits else None
+                if train:
+                    d["out"] = torch.zeros(B, ld, device=dev, dtype=bf)[:, :b.fout]
+                    d["dz"] = torch.zeros(B, ld, device=dev, dtype=bf)[:, :b.fout]
+                    d["mask"] = torch.zeros(B, b.fout, device=dev, dtype=torch.uint8) if b.drop > 0 else None
+                    d["dx_bf16"] = torch.zeros(B, b.fin, device=dev, dtype=bf)
+                else:                                      # the final Linear of the model writes the fp32 logits only
+                    d["out"] = d["logits"] if final_logits else torch.zeros(B, ld, device=dev, dtype=bf)[:, :b.fout]
             self.act.append(d)
-        # gradient w.r.t. the stage output (arrives from the next stage)
-        last = self.act[-1]["out"]
-        self.dout_in = torch.zeros(last.shape, device=dev, dtype=bf)
-        self.dlogits = torch.zeros(B, ex.num_classes, device=dev) if ex.is_last else None
         self.ticket = torch.zeros(4, device=dev, dtype=torch.int32)
         self.tile_counters = torch.zeros(4096, device=dev, dtype=torch.int32)   # split-K tile semaphores (self-resetting)
-        self.gnorm = torch.zeros(4, device=dev)                                 # clip-grad-norm: sum of squared gradients
-        # weight-gradient kernels run on a forked stream: they only feed the optimizer, so they overlap with the
-        # dY -> dX critical path of the layers below (captured as parallel branches of the CUDA graph)
-        self.side = N.new_stream(dev, ex.stream_priority)
+        if train:
+            # gradient w.r.t. the stage output (arrives from the next stage)
+            last = self.act[-1]["out"]
+            self.dout_in = torch.zeros(last.shape, device=dev, dtype=bf)
+            self.dlogits = torch.zeros(B, ex.num_classes, device=dev) if ex.is_last else None
+            self.gnorm = torch.zeros(4, device=dev)                             # clip-grad-norm: sum of squared gradients
+            # weight-gradient kernels run on a forked stream: they only feed the optimizer, so they overlap with the
+            # dY -> dX critical path of the layers below (captured as parallel branches of the CUDA graph)
+            self.side = N.new_stream(dev, ex.stream_priority)
         self.graphs: Dict[Tuple[str, int], torch.cuda.CUDAGraph] = {}
         self._warm = False
 
@@ -565,6 +615,10 @@ class _Plan:
         off, n = self.soff[(bi, name)]
         t = self.scratch[off:off + n]
         return t.view(shape) if shape is not None else t
+
+    def W(self, key: str) -> torch.Tensor:
+        """Weights the GEMMs of this plan read: the executor's choice, or the fp32 master in eval mode."""
+        return self.ex.view(self.ex.P, key) if self.eval else self.ex.W(key)
 
     def acquire_slot(self) -> int:
         if not self.free:
@@ -589,8 +643,10 @@ class _Plan:
     # ---- the kernel sequences ------------------------------------------------------
     def _forward(self, slot: int, out_ptr_override: Optional[torch.Tensor] = None, publish=None, wait=None) -> None:
         """``wait``: (flag_ptr, expect_ctr, max_spins, status) of the mailbox slot this pass consumes — acquired inside the
-        pass's first kernel (the scratch zeroing) instead of a stand-alone wait launch."""
+        pass's first kernel (the scratch zeroing) instead of a stand-alone wait launch.  An eval-mode plan runs the same
+        sequence with BatchNorm on the running statistics (no conv statistics, no fused cut tail) and no dropout."""
         ex = self.ex
+        ev = self.eval
         N.zero_(self.scratch, wait=wait)
         x: torch.Tensor = self.x_in[slot]
         nb = len(ex.blocks)
@@ -603,7 +659,7 @@ class _Plan:
                 if plain:
                     tgt = a["y"] if not (is_final and out_ptr_override is not None) else out_ptr_override
                     facc = self.s(bi, "facc") if (bi, "facc") in self.soff else None
-                    N.conv3x3_fwd(x, ex.W(f"layer{b.conv}.weight"), tgt, ex.view(ex.P, f"layer{b.conv}.bias"),
+                    N.conv3x3_fwd(x, self.W(f"layer{b.conv}.weight"), tgt, ex.view(ex.P, f"layer{b.conv}.bias"),
                                   acc=facc, counters=self.tile_counters)
                     if is_final and publish is not None:
                         N.set_flag(publish["flag"].data_ptr() if hasattr(publish["flag"], "data_ptr") else publish["flag"],
@@ -612,7 +668,7 @@ class _Plan:
                     a["y_eff"] = a["y"]
                     x = tgt
                     continue
-                fuse = (ex.fused_cut and is_final and out_ptr_override is not None and b.conv is not None and b.bn is not None
+                fuse = (ex.fused_cut and not ev and is_final and out_ptr_override is not None and b.conv is not None and b.bn is not None
                         and b.cin > 4 and N.fused_cut_supported(self.B, b.H, b.W, b.cin, b.cout, b.pool, ke=ex.ke))
                 if fuse:
                     # cut-tail kernel: GEMM + BN statistics + BN/ReLU/pool + store into the (peer) mailbox + flag
@@ -633,51 +689,62 @@ class _Plan:
                     x = out_ptr_override
                     continue
                 if b.conv is not None:
-                    s1, s2 = self.s(bi, "sum"), self.s(bi, "sumsq")
+                    s1, s2 = (None, None) if ev else (self.s(bi, "sum"), self.s(bi, "sumsq"))
                     bias = ex.view(ex.P, f"layer{b.conv}.bias")
                     if b.cin <= 4:
                         N.conv3x3_small_fwd(x, ex.view(ex.P, f"layer{b.conv}.weight"), bias, a["y"], s1, s2)
                     else:
                         facc = self.s(bi, "facc") if (bi, "facc") in self.soff else None
-                        N.conv3x3_fwd(x, ex.W(f"layer{b.conv}.weight"), a["y"], bias, s1, s2, acc=facc,
+                        N.conv3x3_fwd(x, self.W(f"layer{b.conv}.weight"), a["y"], bias, s1, s2, acc=facc,
                                       counters=self.tile_counters)
                     y = a["y"]
                 else:
                     y = x
-                    if b.bn is not None:
+                    if b.bn is not None and not ev:
                         s1, s2 = self.s(bi, "sum"), self.s(bi, "sumsq")
                         N.col_stats(y.reshape(-1, b.cout), s1, s2)
                 out = a["out"] if not (is_final and out_ptr_override is not None) else out_ptr_override
                 kw = {}
                 if is_final and publish is not None:
                     kw = dict(ticket=self.ticket, flag=publish["flag"], seq=publish["seq"], hint=publish.get("hint"))
-                if b.bn is not None:
+                if b.bn is not None and ev:
+                    st = ex.bn_state[b.bn]
+                    N.bn_relu_pool_infer(y, ex.view(ex.P, f"layer{b.bn}.weight"), ex.view(ex.P, f"layer{b.bn}.bias"),
+                                         st["running_mean"], st["running_var"], out, b.H, b.W, b.relu, b.pool)
+                elif b.bn is not None:
                     st = ex.bn_state[b.bn]
                     N.bn_relu_pool_fwd(y, self.s(bi, "sum"), self.s(bi, "sumsq"), ex.view(ex.P, f"layer{b.bn}.weight"),
                                        ex.view(ex.P, f"layer{b.bn}.bias"), st["running_mean"], st["running_var"],
                                        st["num_batches_tracked"], a["save_mean"], a["save_invstd"], out, b.H, b.W,
                                        b.relu, b.pool, **kw)
                 else:
-                    N.bn_relu_pool_fwd(y, None, None, None, None, None, None, None, a["save_mean"], a["save_invstd"], out,
-                                       b.H, b.W, b.relu, b.pool, update_running=False, identity=True, **kw)
+                    N.bn_relu_pool_fwd(y, None, None, None, None, None, None, None, a.get("save_mean"), a.get("save_invstd"),
+                                       out, b.H, b.W, b.relu, b.pool, update_running=False, identity=True, **kw)
                 a["y_eff"] = y
                 x = a["out"] if out is a["out"] else out
             elif isinstance(b, DropoutOp):
                 xin = x.reshape(self.B, -1)
                 a["in"] = xin
-                N.dropout_fwd(xin, a["out"], a["mask"], b.p, ex.seed + b.idx, ex.step_ctr)
+                if ev:                                     # inference: dropout is the identity
+                    a["out"] = xin
+                else:
+                    N.dropout_fwd(xin, a["out"], a["mask"], b.p, ex.seed + b.idx, ex.step_ctr)
                 x = a["out"]
             else:
                 xin = x.reshape(self.B, -1)
                 a["in"] = xin
                 acc = self.s(bi, "acc", (self.B, b.fout))
-                w = ex.W(f"layer{b.lin}.weight")
-                if ex.fp32:
+                w = self.W(f"layer{b.lin}.weight")
+                if self.fp32:
                     N.linear_fwd_f32(xin, w, acc)
                 else:
                     N.linear_fwd(xin, w, acc, k_split=max(1, min(8, (b.fin // 64) // 8)))
-                N.linear_finalize(acc, ex.view(ex.P, f"layer{b.lin}.bias"), a["out"], a["logits"], a["mask"], b.relu,
-                                  b.drop, ex.seed + b.lin, ex.step_ctr)
+                if ev:
+                    N.linear_finalize(acc, ex.view(ex.P, f"layer{b.lin}.bias"),
+                                      None if a["out"] is a["logits"] else a["out"], a["logits"], None, b.relu)
+                else:
+                    N.linear_finalize(acc, ex.view(ex.P, f"layer{b.lin}.bias"), a["out"], a["logits"], a["mask"], b.relu,
+                                      b.drop, ex.seed + b.lin, ex.step_ctr)
                 x = a["out"]
 
     def _backward(self, dout: torch.Tensor, grad_out_override: Optional[torch.Tensor] = None, publish_grad=None) -> None:
@@ -841,6 +908,15 @@ class _Plan:
 
     def run_last(self) -> None:
         self._exec(("last", 0), lambda: self._last())
+
+    def run_eval(self, metrics=None) -> None:
+        """Eval-mode forward of ``x_in[0]``; ``metrics = (loss_total, correct, count)`` device accumulators: the same graph
+        also adds this batch's loss / accuracy against ``labels`` (last stage only)."""
+        def body():
+            self._forward(0)
+            if metrics is not None:
+                N.eval_metrics(self.act[-1]["logits"], self.labels, *metrics)
+        self._exec(("eval", int(metrics is not None)), body)
 
     def _exec(self, key, fn) -> None:
         ex = self.ex

@@ -6,17 +6,24 @@ means + accuracy, logged through the server logger.  ``get_val`` returns ``(ok, 
 (other/Vanilla_SL/src/Validation.py:46,55-56).  ``pump`` is called every 5 batches — the
 hook DCSL uses to keep its AMQP heartbeat alive (other/DCSL/src/Validation.py:48-52); here it
 lets the broker thread breathe / watchdogs tick.
+
+``native`` (``b200.native-validation``) selects the backend: ``false`` (default) the torch modules above; ``true`` the
+native eval plan (``train/b200_eval.py``) on the test split resident in HBM, an error where there is none; ``auto`` native
+where supported, torch otherwise with one log line giving the reason.  Metrics carry ``val_backend``.
 """
 from __future__ import annotations
 
+import logging
 import math
-from typing import Callable, Dict, Optional, Tuple
+from typing import Any, Callable, Dict, Optional, Tuple
 
 import torch
 import torch.nn as nn
 
 from .data import data_loader
 from .models import get_model_class
+
+_NATIVE: Dict[Tuple, Any] = {}          # (model, data, device, synthetic) -> (NativeEvaluator, resident test split)
 
 
 @torch.no_grad()
@@ -42,18 +49,81 @@ def evaluate(model: nn.Module, loader, device, pump: Optional[Callable[[], None]
             "val_correct": correct, "val_total": total}
 
 
+def native_mode(native) -> str:
+    """Normalise a ``b200.native-validation`` value to "false" | "true" | "auto"."""
+    if native is None or isinstance(native, bool):
+        return "true" if native else "false"
+    s = str(native).strip().lower()
+    if s in ("false", "0", "no", "off", ""):
+        return "false"
+    if s in ("true", "1", "yes", "on"):
+        return "true"
+    if s == "auto":
+        return "auto"
+    raise ValueError(f"b200.native-validation must be true, false or auto, got {native!r}")
+
+
+def native_unsupported_reason(klass, data_name: str, device) -> Optional[str]:
+    """Why the native evaluator cannot run this (model, data, device) — None when it can."""
+    dev = torch.device(device)
+    if dev.type != "cuda" or not torch.cuda.is_available():
+        return "no CUDA device"
+    if str(data_name).upper() != "CIFAR10":
+        return f"no resident test split for {data_name}"
+    from .train.b200_eval import native_eval_supported
+    if not native_eval_supported(klass):
+        return f"{klass.__name__} has no native eval plan"
+    return None
+
+
+def _native_evaluate(klass, model_name, data_name, state_dict_full, device, pump, synthetic) -> Dict[str, float]:
+    from .data import resident_test_loader
+    from .train.b200_eval import NativeEvaluator
+    dev = torch.device(device)
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    key = (model_name, str(data_name).upper(), str(dev), synthetic)
+    hit = _NATIVE.get(key)
+    if hit is None:
+        hit = _NATIVE[key] = (NativeEvaluator(klass, state_dict_full, dev), resident_test_loader(data_name, dev, synthetic))
+    else:
+        hit[0].load_state_dict(state_dict_full)
+    evaluator, source = hit
+    return evaluator.evaluate(source, pump)
+
+
 def get_val(model_name: str, data_name: str, state_dict_full, logger=None, strict: bool = False,
-            device: Optional[str] = None, pump=None, synthetic: Optional[bool] = None) -> Tuple[bool, Dict[str, float]]:
+            device: Optional[str] = None, pump=None, synthetic: Optional[bool] = None,
+            native=False) -> Tuple[bool, Dict[str, float]]:
     try:
         klass = get_model_class(model_name, data_name)
     except ValueError:
         return False, {}
     device = device or ("cuda" if torch.cuda.is_available() else "cpu")
-    model = klass()
-    model.load_state_dict(state_dict_full)
-    model.to(device)
-    loader = data_loader(data_name=data_name, train=False, synthetic=synthetic)
-    m = evaluate(model, loader, device, pump)
+    mode = native_mode(native)
+    backend = "torch"
+    if mode != "false":
+        reason = native_unsupported_reason(klass, data_name, device)
+        if reason is None:
+            backend = "native"
+        elif mode == "true":
+            raise RuntimeError(f"b200.native-validation is true but {model_name}/{data_name} on {device} cannot run "
+                               f"natively: {reason}")
+        else:
+            line = f"native validation unavailable ({reason}): validating with torch"
+            if logger is not None:
+                logger.log_info(line)
+            else:
+                logging.getLogger(__name__).info(line)
+    if backend == "native":
+        m = _native_evaluate(klass, model_name, data_name, state_dict_full, device, pump, synthetic)
+    else:
+        model = klass()
+        model.load_state_dict(state_dict_full)
+        model.to(device)
+        loader = data_loader(data_name=data_name, train=False, synthetic=synthetic)
+        m = evaluate(model, loader, device, pump)
+    m["val_backend"] = backend
     line = "Test set:Loss: {:.4f}; Accuracy: {}/{} ({:.2f}%)\n".format(
         m["val_loss"], m["val_correct"], m["val_total"], m["val_acc"])
     if logger is not None:
