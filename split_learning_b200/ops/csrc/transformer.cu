@@ -587,14 +587,24 @@ static int check_launch() {
   return e == cudaSuccess ? 0 : -static_cast<int>(e) - 2000;
 }
 
+// The heads of one operand, columns [col + h * Dh, col + (h + 1) * Dh) for h < H, must each lie inside one 64-column
+// TMA box (the kernel loads the box at col & ~63 and walks Dh columns from col & 63), and inside the row pitch (past
+// it TMA would read zero fill and the head would be silently wrong).  Dh divides 64, so col % Dh == 0 keeps every
+// head inside its box.
+static bool heads_fit(int col, int H, int Dh, long long ld) {
+  return col >= 0 && col % Dh == 0 && col + static_cast<long long>(H) * Dh <= ld;
+}
+
 extern "C" {
 
 // q/k/v: bf16 [B*S][ld*]; head h of Q lives at columns q_col + h*Dh ...  out: [B*S][ldo]; lse: [B*H][128] fp32
 int slb_attn_fwd(const void* q, const void* k, const void* v, long long ldq, long long ldk, long long ldv, int q_col,
                  int k_col, int v_col, void* out, long long ldo, float* lse, const float* key_bias, int B, int S, int H,
                  int Dh, float p_drop, unsigned seed, const unsigned* seed_ofs, cudaStream_t st) {
-  if (S < 1 || S > 128 || (Dh != 32 && Dh != 64)) return -3;
-  if ((q_col | k_col | v_col) & 31 || ((ldq | ldk | ldv | ldo) & 7)) return -4;
+  if (B < 1 || H < 1 || S < 1 || S > 128 || (Dh != 32 && Dh != 64)) return -3;
+  if (((ldq | ldk | ldv | ldo) & 7) || !heads_fit(q_col, H, Dh, ldq) || !heads_fit(k_col, H, Dh, ldk) ||
+      !heads_fit(v_col, H, Dh, ldv) || static_cast<long long>(H) * Dh > ldo)
+    return -4;
   CUtensorMap tq, tk, tv;
   const uint64_t rows = static_cast<uint64_t>(B) * S;
   int r;
@@ -620,9 +630,12 @@ int slb_attn_bwd(const void* q, const void* k, const void* v, const void* dout, 
                  long long lddq, long long lddk, long long lddv, int dq_col, int dk_col, int dv_col, const float* lse,
                  const float* key_bias, int B, int S, int H, int Dh, float p_drop, unsigned seed, const unsigned* seed_ofs,
                  cudaStream_t st) {
-  if (S < 1 || S > 128 || (Dh != 32 && Dh != 64)) return -3;
-  if ((q_col | k_col | v_col | do_col) & 31 || ((ldq | ldk | ldv | lddo | lddq | lddk | lddv) & 7) ||
-      ((dq_col | dk_col | dv_col) & 7))
+  if (B < 1 || H < 1 || S < 1 || S > 128 || (Dh != 32 && Dh != 64)) return -3;
+  const long long width = static_cast<long long>(H) * Dh;
+  if (((ldq | ldk | ldv | lddo | lddq | lddk | lddv) & 7) || ((dq_col | dk_col | dv_col) & 7) ||
+      !heads_fit(q_col, H, Dh, ldq) || !heads_fit(k_col, H, Dh, ldk) || !heads_fit(v_col, H, Dh, ldv) ||
+      !heads_fit(do_col, H, Dh, lddo) || dq_col < 0 || dk_col < 0 || dv_col < 0 || dq_col + width > lddq ||
+      dk_col + width > lddk || dv_col + width > lddv)
     return -4;
   CUtensorMap tq, tk, tv, tdo;
   const uint64_t rows = static_cast<uint64_t>(B) * S;

@@ -78,6 +78,13 @@ struct GemmParams {
   Det det;                        // reproducible reductions: BN statistics across m-tiles, split-K turns without tile_counters
 };
 
+// May 32 columns at `ptr` be moved as 16-byte vectors?  Conv and wgrad rows always start 16-byte aligned (the host
+// requires Nout % 32 == 0), so only MODE_GEMM tests the pointer: its ldo is free (a Linear with 36 or 100 outputs).
+template <int MODE>
+__device__ __forceinline__ bool vec16_ok(const void* ptr) {
+  return MODE != MODE_GEMM || (reinterpret_cast<uintptr_t>(ptr) & 15) == 0;
+}
+
 __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == 1) return fmaxf(x, 0.f);
   if (act == 2) return 0.5f * x * (1.f + erff(x * 0.70710678118654752f));
@@ -402,7 +409,7 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if constexpr (MODE == MODE_GEMM && !OT::TF32) {
             if (p.residual != nullptr && row_store) {
               const __nv_bfloat16* rs = p.residual + row_off + col0;
-              if (col0 + 32 <= p.N) {
+              if (col0 + 32 <= p.N && vec16_ok<MODE>(rs)) {
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                   const uint4 u = __ldg(reinterpret_cast<const uint4*>(rs) + j);
@@ -421,7 +428,7 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) f[j] += __bfl
             }
             if (p.aux_out != nullptr && row_store) {
               __nv_bfloat16* ao = p.aux_out + row_off + col0;
-              if (col0 + 32 <= p.N) {
+              if (col0 + 32 <= p.N && vec16_ok<MODE>(ao)) {
                 uint4* a4 = reinterpret_cast<uint4*>(ao);
 #pragma unroll
                 for (int j = 0; j < 4; ++j)
@@ -439,7 +446,7 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) ao[j] = __flo
           }
           if (row_store) {
             T* o = reinterpret_cast<T*>(p.out) + row_off + col0;
-            if (col0 + 32 <= p.N) {
+            if (col0 + 32 <= p.N && vec16_ok<MODE>(o)) {   // tf32 (T = float) outputs are conv / wgrad only: aligned
               store_row32(o, f);
             } else {
               {
@@ -493,7 +500,7 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = static
         } else {  // EPI_F32_STORE
           if (row_store) {
             float* o = reinterpret_cast<float*>(p.out) + row_off + col0;
-            if (col0 + 32 <= p.N) {
+            if (col0 + 32 <= p.N && vec16_ok<MODE>(o)) {
               float4* o4 = reinterpret_cast<float4*>(o);
 #pragma unroll
               for (int j = 0; j < 8; ++j)
@@ -536,6 +543,7 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = __uint
             }
 #pragma unroll
             for (int j = 0; j < 32; ++j) f[j] += s_bias[c + j];
+            // fin_out / fin_ld exist for the conv split-K path only, where fin_ld = Nout % 32 == 0: rows stay aligned
             if (row_ok) store_row32(reinterpret_cast<T*>(p.fin_out) + static_cast<long long>(row) * p.fin_ld + col0, f);
             if (want_stats) {
               float c1, c2;

@@ -518,24 +518,26 @@ def _gemm_bn(n: int, m: int, b_mn: bool = False) -> int:
 
 
 def gemm_act(a, b, out, M, N, K, a_mn=False, b_mn=False, lda=None, ldb=None, ldo=None, bias=None, act=None, aux=None,
-             residual=None):
+             residual=None, block_n=None):
     """out_bf16[M, N] = act(A B^T + bias + residual).  A: [M, K] (K-major) or [K, M] storage (``a_mn``);
-    B: [N, K] (K-major) or [K, N] storage (``b_mn``).  ``aux`` receives the pre-activation."""
+    B: [N, K] (K-major) or [K, N] storage (``b_mn``).  ``aux`` receives the pre-activation.  ``block_n`` forces the
+    column-tile width (32 / 64 / 128 / 256; 32 is K-major B only); the default picks it from the shape."""
     lda = lda if lda is not None else (M if a_mn else K)
     ldb = ldb if ldb is not None else (N if b_mn else K)
     ldo = ldo if ldo is not None else N
-    bn = _gemm_bn(N, M, b_mn)
+    bn = block_n if block_n is not None else _gemm_bn(N, M, b_mn)
     _check(lib().slb_gemm_bf16_act(_p(a), _p(b), _p(out), c_int(M), c_int(N), c_int(K), c_int(int(a_mn)), c_int(int(b_mn)),
                                    c_longlong(lda), c_longlong(ldb), c_longlong(ldo), c_int(bn), _p(bias), c_int(ACT[act]),
                                    _p(aux), _p(residual), _stream()), "gemm_act")
 
 
-def gemm_f32(a, b, out, M, N, K, a_mn=False, b_mn=False, lda=None, ldb=None, ldo=None, k_split=1):
-    """out_fp32[M, N] += A B^T (fp32 red.add epilogue: accumulates into a live gradient buffer, any ``k_split``)."""
+def gemm_f32(a, b, out, M, N, K, a_mn=False, b_mn=False, lda=None, ldb=None, ldo=None, k_split=1, block_n=None):
+    """out_fp32[M, N] += A B^T (fp32 red.add epilogue: accumulates into a live gradient buffer, any ``k_split``).
+    ``block_n`` as for ``gemm_act``."""
     lda = lda if lda is not None else (M if a_mn else K)
     ldb = ldb if ldb is not None else (N if b_mn else K)
     ldo = ldo if ldo is not None else N
-    bn = _gemm_bn(N, M, b_mn)
+    bn = block_n if block_n is not None else _gemm_bn(N, M, b_mn)
     _check(lib().slb_gemm_bf16(_p(a), _p(b), _p(out), c_int(M), c_int(N), c_int(K), c_int(int(a_mn)), c_int(int(b_mn)),
                                c_longlong(lda), c_longlong(ldb), c_longlong(ldo), c_int(1), c_int(max(1, k_split)), c_int(bn),
                                _stream()), "gemm_f32")
