@@ -888,9 +888,24 @@ __device__ __forceinline__ uint32_t hash_u32(uint32_t a, uint32_t b, uint32_t c)
   h ^= h >> 16; h *= 0x7FEB352Du; h ^= h >> 15; h *= 0x846CA68Bu; h ^= h >> 16;
   return h;
 }
+// Value i of a sliced fp32 Linear result (linear_fwd_f32 / linear_dgrad_f32): +0 plus the `parts` slice partials
+// p[i + z * stride] in slice order, each added with add.rn.ftz — the arithmetic of red.global.add.f32 into a zeroed buffer
+// in slice order, so the sum is the same every run without the slices waiting for one another.  parts == 0: p[i] is final.
+__device__ __forceinline__ float slice_sum(const float* p, long long stride, int parts, long long i) {
+  if (parts == 0) return p[i];
+  float s = 0.f;
+#pragma unroll 8
+  for (int z = 0; z < parts; ++z) {
+    const float v = p[i + z * stride];
+    asm("add.rn.ftz.f32 %0, %0, %1;" : "+f"(s) : "f"(v));
+  }
+  return s;
+}
+
 // out[b][n] = dropout(relu(acc[b][n] + bias[n]))  -> activation type (ld = ldo) ; also keeps fp32 logits when out_f32 != null
+// acc: `parts` slice partials [parts][B][N] (slice_sum)
 template <typename T>
-__global__ void linear_finalize_kernel(const float* acc, const float* bias, T* out, float* out_f32, uint8_t* mask,
+__global__ void linear_finalize_kernel(const float* acc, int parts, const float* bias, T* out, float* out_f32, uint8_t* mask,
                                        int B, int N, int ldo, int relu, float drop_p, uint32_t seed, const uint32_t* step_ptr) {
   pdl_trigger();
   pdl_wait();
@@ -900,7 +915,7 @@ __global__ void linear_finalize_kernel(const float* acc, const float* bias, T* o
   const uint32_t thresh = static_cast<uint32_t>(drop_p * 4294967296.0);
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int n = static_cast<int>(i % N), b = static_cast<int>(i / N);
-    float v = acc[i] + (bias ? bias[n] : 0.f);
+    float v = slice_sum(acc, total, parts, i) + (bias ? bias[n] : 0.f);
     if (relu) v = fmaxf(v, 0.f);
     if (drop_p > 0.f) {
       const bool keep = hash_u32(seed, step, static_cast<uint32_t>(i)) >= thresh;
@@ -914,7 +929,7 @@ __global__ void linear_finalize_kernel(const float* acc, const float* bias, T* o
 // dz[b][n] = dy[b][n] * dropmask * (relu ? y>0 : 1)  (bf16, ld = ldz) ; db[n] = sum_b dz[b][n] (bf16-rounded values)
 // blockDim = (32 columns, 8 row groups): rows are split over threadIdx.y, the bias gradient is combined in smem
 template <typename T>
-__global__ void __launch_bounds__(256) linear_bwd_prep_kernel(const float* dacc, const T* yout, const uint8_t* mask,
+__global__ void __launch_bounds__(256) linear_bwd_prep_kernel(const float* dacc, int parts, const T* yout, const uint8_t* mask,
                                                              T* dz, float* dbias, int B, int N, int ldy, int ldz,
                                                              int relu, float drop_p) {
   pdl_trigger();
@@ -925,7 +940,7 @@ __global__ void __launch_bounds__(256) linear_bwd_prep_kernel(const float* dacc,
   float s = 0.f;
   if (n < N) {
     for (int b = threadIdx.y; b < B; b += 8) {
-      float g = dacc[(long long)b * N + n];
+      float g = slice_sum(dacc, (long long)B * N, parts, (long long)b * N + n);
       if (drop_p > 0.f) g = mask[(long long)b * N + n] ? g * keep_scale : 0.f;
       if (relu && !(to_f32(yout[(long long)b * ldy + n]) > 0.f)) g = 0.f;
       const T r = from_f32<T>(g);
@@ -958,12 +973,12 @@ __global__ void dropout_fwd_kernel(const T* x, T* y, uint8_t* mask, long long n,
   }
 }
 template <typename T>
-__global__ void dropout_bwd_kernel(const float* dacc, const uint8_t* mask, T* dx, long long n, float p) {
+__global__ void dropout_bwd_kernel(const float* dacc, int parts, const uint8_t* mask, T* dx, long long n, float p) {
   pdl_trigger();
   pdl_wait();
   const float ks = 1.f / (1.f - p);
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    dx[i] = from_f32<T>((mask == nullptr || mask[i]) ? dacc[i] * (mask ? ks : 1.f) : 0.f);
+    dx[i] = from_f32<T>((mask == nullptr || mask[i]) ? slice_sum(dacc, n, parts, i) * (mask ? ks : 1.f) : 0.f);
 }
 
 
@@ -1000,12 +1015,11 @@ __device__ __forceinline__ f32x2 ffma2(f32x2 a, f32x2 b, f32x2 c) {
   return pack2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 
-// acc[b][n] (+)= sum_{k in slice} x[b][k] * w[n][k]            grid (ceil(N/32), ceil(K/kc), ceil(B/32)), 256 threads
+// part[s][b][n] = sum_{k in slice s} x[b][k] * w[n][k]          grid (ceil(N/32), ceil(K/kc), ceil(B/32)), 256 threads
 // warp = (feature group of 8) x (batch half of 16); lanes stride K in float4 steps; partial sums are reduced across the
-// warp with the register butterfly and added to `acc` (zeroed by the caller) with one atomic per (b, n) per slice.
+// warp with the register butterfly and stored as slice s's partial (the consumer adds the slices in order: slice_sum).
 __global__ void __launch_bounds__(256) linear_fwd_f32_kernel(const float* __restrict__ x, const float* __restrict__ w,
-                                                            float* acc, int B, int N, int K, int ldx, int ldw, int lda, int kc,
-                                                            const Det det) {
+                                                            float* part, int B, int N, int K, int ldx, int ldw, int kc) {
   pdl_trigger();
   pdl_wait();
   constexpr int ST = 4;                                          // weight stages in flight (16 KB each)
@@ -1097,30 +1111,20 @@ __global__ void __launch_bounds__(256) linear_fwd_f32_kernel(const float* __rest
   float v[4];
 #pragma unroll
   for (int q = 0; q < 4; ++q) v[q] = warp_col_reduce32e(a[q]);  // lane j: sum over lanes of a[q][j]
-  // K slices add in slice order (blockIdx.y) behind a turn counter: the same sum every run
-  uint32_t* turn = det.ctr + DET_TURN_BASE + blockIdx.z * gridDim.x + blockIdx.x;
-  if (gridDim.y > 1) {
-    if (threadIdx.x == 0) turn_wait(turn, blockIdx.y);
-    __syncthreads();
-  }
+  float* ps = part + (long long)blockIdx.y * B * N;
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     const int f = 2 * q + (lane >> 4), b = b0 + bh * 16 + (lane & 15);
-    if (n0 + f < N && b < B) atomicAdd(acc + (long long)b * lda + n0 + f, v[q]);
-  }
-  if (gridDim.y > 1) {
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) turn_pass(turn, blockIdx.y, gridDim.y);
+    if (n0 + f < N && b < B) ps[(long long)b * N + n0 + f] = v[q];
   }
 }
 
-// dacc[b][k] += sum_{n in slice} dz[b][n] * w[n][k]            grid (ceil(K/(4*T)), ceil(N/nc), ceil(B/32)), T threads
+// part[s][b][k] = sum_{n in slice s} dz[b][n] * w[n][k]         grid (ceil(K/(4*T)), ceil(N/nc), ceil(B/32)), T threads
 // a thread owns 4 consecutive k for the whole batch tile (128 accumulators); the dz slice sits in shared memory as
 // [n][32 b] and is read with warp-broadcast 16-byte loads; weights stream through with coalesced float4 loads.
-__global__ void __launch_bounds__(128) linear_dgrad_f32_kernel(const float* __restrict__ dz, const float* __restrict__ w, float* dacc,
-                                                              int B, int N, int K, int lddz, int ldw, int ldd, int nc,
-                                                              const Det det) {
+// The consumer adds the slices in order (slice_sum).
+__global__ void __launch_bounds__(128) linear_dgrad_f32_kernel(const float* __restrict__ dz, const float* __restrict__ w, float* part,
+                                                              int B, int N, int K, int lddz, int ldw, int nc) {
   pdl_trigger();
   pdl_wait();
   extern __shared__ __align__(16) float s_dz[];                  // [nc][32]
@@ -1181,23 +1185,11 @@ __global__ void __launch_bounds__(128) linear_dgrad_f32_kernel(const float* __re
   for (int bp = 0; bp < 16; ++bp)
 #pragma unroll
     for (int k = 0; k < 4; ++k) unpack2(acc[bp][k], a[2 * bp][k], a[2 * bp + 1][k]);
-  // N slices add in slice order (blockIdx.y) behind a turn counter: the same sum every run
-  uint32_t* turn = det.ctr + DET_TURN_BASE + blockIdx.z * gridDim.x + blockIdx.x;
-  if (gridDim.y > 1) {
-    if (threadIdx.x == 0) turn_wait(turn, blockIdx.y);
-    __syncthreads();
-  }
+  float* ps = part + (long long)blockIdx.y * B * K;
 #pragma unroll
   for (int b = 0; b < 32; ++b)
     if (b0 + b < B)
-      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dacc + (long long)(b0 + b) * ldd + k0), "f"(a[b][0]),
-                   "f"(a[b][1]), "f"(a[b][2]), "f"(a[b][3])
-                   : "memory");
-  if (gridDim.y > 1) {
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) turn_pass(turn, blockIdx.y, gridDim.y);
-  }
+      *reinterpret_cast<float4*>(ps + (long long)(b0 + b) * K + k0) = make_float4(a[b][0], a[b][1], a[b][2], a[b][3]);
 }
 
 // g[n][k] = sum_b dz[b][n] * x[b][k]  (K = batch: the weight gradient is written exactly once, so the optimizer step
@@ -1807,23 +1799,27 @@ int slb_conv3x3_small_wgrad(const float* x, const void* dy, float* dw, int B, in
                     : small_wgrad_t<__nv_bfloat16>(x, dy, dw, B, Cin, H, W, Cout, st);
 }
 
-int slb_linear_finalize(const float* acc, const float* bias, void* out, float* out_f32, uint8_t* mask, int B, int N, int ldo,
-                        int relu, float drop_p, uint32_t seed, const uint32_t* step_ptr, int dtype, cudaStream_t st) {
+// acc / dacc below: `parts` slice partials [parts][B][N] of linear_fwd_f32 / linear_dgrad_f32, summed in slice order, or
+// (parts == 0) one finished [B][N] buffer
+int slb_linear_finalize(const float* acc, int parts, const float* bias, void* out, float* out_f32, uint8_t* mask, int B, int N,
+                        int ldo, int relu, float drop_p, uint32_t seed, const uint32_t* step_ptr, int dtype, cudaStream_t st) {
+  if (parts < 0) return -1;
   if (dtype == 1)
-    launch_k(linear_finalize_kernel<float>, grid_for((long long)B * N, 256), 256, 0, st, acc, bias, reinterpret_cast<float*>(out),
-             out_f32, mask, B, N, ldo, relu, drop_p, seed, step_ptr);
+    launch_k(linear_finalize_kernel<float>, grid_for((long long)B * N, 256), 256, 0, st, acc, parts, bias,
+             reinterpret_cast<float*>(out), out_f32, mask, B, N, ldo, relu, drop_p, seed, step_ptr);
   else
-    launch_k(linear_finalize_kernel<__nv_bfloat16>, grid_for((long long)B * N, 256), 256, 0, st, acc, bias,
+    launch_k(linear_finalize_kernel<__nv_bfloat16>, grid_for((long long)B * N, 256), 256, 0, st, acc, parts, bias,
              reinterpret_cast<__nv_bfloat16*>(out), out_f32, mask, B, N, ldo, relu, drop_p, seed, step_ptr);
   return last_err();
 }
-int slb_linear_bwd_prep(const float* dacc, const void* yout, const uint8_t* mask, void* dz, float* dbias, int B, int N, int ldy,
-                        int ldz, int relu, float drop_p, int dtype, cudaStream_t st) {
+int slb_linear_bwd_prep(const float* dacc, int parts, const void* yout, const uint8_t* mask, void* dz, float* dbias, int B, int N,
+                        int ldy, int ldz, int relu, float drop_p, int dtype, cudaStream_t st) {
+  if (parts < 0) return -1;
   if (dtype == 1)
-    launch_k(linear_bwd_prep_kernel<float>, (N + 31) / 32, dim3(32, 8), 0, st, dacc, reinterpret_cast<const float*>(yout), mask,
-             reinterpret_cast<float*>(dz), dbias, B, N, ldy, ldz, relu, drop_p);
+    launch_k(linear_bwd_prep_kernel<float>, (N + 31) / 32, dim3(32, 8), 0, st, dacc, parts, reinterpret_cast<const float*>(yout),
+             mask, reinterpret_cast<float*>(dz), dbias, B, N, ldy, ldz, relu, drop_p);
   else
-    launch_k(linear_bwd_prep_kernel<__nv_bfloat16>, (N + 31) / 32, dim3(32, 8), 0, st, dacc,
+    launch_k(linear_bwd_prep_kernel<__nv_bfloat16>, (N + 31) / 32, dim3(32, 8), 0, st, dacc, parts,
              reinterpret_cast<const __nv_bfloat16*>(yout), mask, reinterpret_cast<__nv_bfloat16*>(dz), dbias, B, N, ldy, ldz, relu,
              drop_p);
   return last_err();
@@ -1838,42 +1834,64 @@ int slb_dropout_fwd(const void* x, void* y, uint8_t* mask, long long n, float p,
              reinterpret_cast<__nv_bfloat16*>(y), mask, n, p, seed, step_ptr);
   return last_err();
 }
-int slb_dropout_bwd(const float* dacc, const uint8_t* mask, void* dx, long long n, float p, int dtype, cudaStream_t st) {
-  if (dtype == 1) launch_k(dropout_bwd_kernel<float>, grid_for(n, 256), 256, 0, st, dacc, mask, reinterpret_cast<float*>(dx), n, p);
-  else launch_k(dropout_bwd_kernel<__nv_bfloat16>, grid_for(n, 256), 256, 0, st, dacc, mask, reinterpret_cast<__nv_bfloat16*>(dx), n, p);
+int slb_dropout_bwd(const float* dacc, int parts, const uint8_t* mask, void* dx, long long n, float p, int dtype, cudaStream_t st) {
+  if (parts < 0) return -1;
+  if (dtype == 1)
+    launch_k(dropout_bwd_kernel<float>, grid_for(n, 256), 256, 0, st, dacc, parts, mask, reinterpret_cast<float*>(dx), n, p);
+  else
+    launch_k(dropout_bwd_kernel<__nv_bfloat16>, grid_for(n, 256), 256, 0, st, dacc, parts, mask,
+             reinterpret_cast<__nv_bfloat16*>(dx), n, p);
   return last_err();
 }
 
-// ---- fp32 Linear (CUDA cores).  K % 4 == 0 and 16-byte aligned rows required.
-int slb_linear_fwd_f32(const float* x, const float* w, float* acc, int B, int N, int K, int ldx, int ldw, int lda, cudaStream_t st) {
-  if (K % 4 || ldx % 4 || ldw % 4) return -1;
-  // K slices: enough CTAs for >= 2 waves when the layer allows, at least 128 k per slice
+// ---- fp32 Linear (CUDA cores).  K % 4 == 0 and 16-byte aligned rows required.  Both kernels store one partial per slice
+// into part[slices][B][out] (no atomics, no zeroing); `part_cap` is the buffer's size in floats.
+// forward, K slices: enough CTAs for >= 2 waves when the layer allows, at least 128 k per slice
+static int linear_fwd_kc(int N, int K) {
   const int fgroups = (N + 31) / 32;
   int kc = 1024;
   while (kc > 128 && fgroups * ((K + kc - 1) / kc) < 296) kc >>= 1;
-  dim3 grid(fgroups, (K + kc - 1) / kc, (B + 31) / 32);
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(linear_fwd_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 32 * 128 * 4); attr = true; }
-  const Det det = slb_det(st);
-  if (det.part == nullptr || (long long)grid.x * grid.z > DET_COUNTERS - DET_TURN_BASE) return -30;
-  launch_k(linear_fwd_f32_kernel, grid, dim3(256), (size_t)4 * 32 * 128 * sizeof(float), st, x, w, acc, B, N, K, ldx, ldw, lda, kc,
-           det);
-  return last_err();
+  return kc;
 }
-int slb_linear_dgrad_f32(const float* dz, const float* w, float* dacc, int B, int N, int K, int lddz, int ldw, int ldd,
-                         cudaStream_t st) {
-  if (K % 4 || ldw % 4 || ldd % 4) return -1;
-  const int threads = K >= 512 ? 128 : 64;
+static int linear_dgrad_threads(int K) { return K >= 512 ? 128 : 64; }
+// input gradient, N slices of nc rows
+static int linear_dgrad_nc(int N, int K) {
+  const int threads = linear_dgrad_threads(K);
   const int ktiles = (K / 4 + threads - 1) / threads;
   int nc = 256;
   while (nc > 32 && ktiles * ((N + nc - 1) / nc) < 296) nc >>= 1;
+  return nc;
+}
+// number of slice partials the forward (dgrad = 0) or input-gradient (dgrad = 1) kernel writes; N = out, K = in features
+int slb_linear_f32_slices(int dgrad, int N, int K) {
+  if (N < 1 || K < 1) return -1;
+  if (dgrad) { const int nc = linear_dgrad_nc(N, K); return (N + nc - 1) / nc; }
+  const int kc = linear_fwd_kc(N, K);
+  return (K + kc - 1) / kc;
+}
+int slb_linear_fwd_f32(const float* x, const float* w, float* part, long long part_cap, int B, int N, int K, int ldx, int ldw,
+                       cudaStream_t st) {
+  if (K % 4 || ldx % 4 || ldw % 4) return -1;
+  const int kc = linear_fwd_kc(N, K);
+  dim3 grid((N + 31) / 32, (K + kc - 1) / kc, (B + 31) / 32);
+  if ((long long)grid.y * B * N > part_cap) return -3;
+  static bool attr = false;
+  if (!attr) { cudaFuncSetAttribute(linear_fwd_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 32 * 128 * 4); attr = true; }
+  launch_k(linear_fwd_f32_kernel, grid, dim3(256), (size_t)4 * 32 * 128 * sizeof(float), st, x, w, part, B, N, K, ldx, ldw, kc);
+  return last_err();
+}
+int slb_linear_dgrad_f32(const float* dz, const float* w, float* part, long long part_cap, int B, int N, int K, int lddz, int ldw,
+                         cudaStream_t st) {
+  if (K % 4 || ldw % 4 || (reinterpret_cast<uintptr_t>(part) & 15)) return -1;
+  const int threads = linear_dgrad_threads(K);
+  const int ktiles = (K / 4 + threads - 1) / threads;
+  const int nc = linear_dgrad_nc(N, K);
   dim3 grid(ktiles, (N + nc - 1) / nc, (B + 31) / 32);
+  if ((long long)grid.y * B * K > part_cap) return -3;
   const size_t smem = (size_t)nc * 32 * sizeof(float) + (size_t)6 * 4 * threads * 16;      // dz slice + per-thread weight ring
   static bool attr = false;
   if (!attr) { cudaFuncSetAttribute(linear_dgrad_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024); attr = true; }
-  const Det det = slb_det(st);
-  if (det.part == nullptr || (long long)grid.x * grid.z > DET_COUNTERS - DET_TURN_BASE) return -30;
-  launch_k(linear_dgrad_f32_kernel, grid, dim3(threads), smem, st, dz, w, dacc, B, N, K, lddz, ldw, ldd, nc, det);
+  launch_k(linear_dgrad_f32_kernel, grid, dim3(threads), smem, st, dz, w, part, B, N, K, lddz, ldw, nc);
   return last_err();
 }
 // mode 0: G = g, 1: G += g, 2: fused SGD-momentum on (P, M) [+ bias rows].  Batches > 32 are looped here (mode 2 needs B <= 32).

@@ -366,7 +366,12 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
 // Float atomics add in whatever order the blocks arrive, so sums differed in their last bits from run to run and a training
 // run drifted apart.  Every cross-block float reduction goes through one of these two orders instead:
 //   det_commit  many blocks: block m of a group stores its partial row, the last block to arrive sums the rows in m order;
-//   turn_*      few slices (split-K): slice z adds its partial into the output after slice z - 1 has (a turn counter).
+//   turn_*      few slices whose caller owns no partial buffer (conv weight gradient, bf16 GEMM split-K, conv split-K
+//               finalised by a separate kernel, loss rows): slice z adds its partial into the output after slice z - 1 has
+//               (a turn counter).  Every hand-off is a serial L2 round trip while the waiting CTAs hold their SMs.
+// Split-K slices with a partial buffer (conv fwd / dgrad with tile_counters, the fp32 Linear kernels) store their partials
+// instead, and one reader adds them in slice order with add.rn.ftz — the arithmetic of red.add.f32 into a zeroed buffer:
+// the last slice of a tile to arrive (umma_gemm.cu) or the whole-grid consumer (elementwise.cu slice_sum).
 // Both rely on blocks of lower linear index being scheduled no later than higher ones.  Counters are zero at rest: the last
 // participant resets them.  Scratch and counters belong to a stream (kernels of one stream never overlap their reductions).
 struct Det {
@@ -375,7 +380,7 @@ struct Det {
   long long cap;        // floats in `part`
 };
 constexpr int DET_COUNTERS = 4096;
-constexpr int DET_TURN_BASE = 64;             // counters [0, 64): det_commit groups; [64, 4096): split-K turns
+constexpr int DET_TURN_BASE = 64;             // counters [0, 64): det_commit groups; [64, 4096): turn counters
 Det slb_det(cudaStream_t st);                 // elementwise.cu; part == nullptr when the scratch could not be allocated
 void slb_det_release(cudaStream_t st);        // frees the stream's scratch (before the stream is destroyed)
 

@@ -49,8 +49,8 @@ struct GemmParams {
   int flip;             // 1: dgrad (mirrored taps)
   int b_row_stride;     // conv: columns of B per tap (= Cin of the weight tensor)
   int Cout;             // wgrad: number of output channels (rows per tap)
-  // split-K with in-kernel finalisation: the last K-slice of a tile to finish converts the fp32 partial sums
-  // (accumulated with red.add in `out`) into the bf16 result + BN statistics — no separate finalize launch.
+  // split-K with in-kernel finalisation: the last K-slice of a tile to arrive adds the fp32 partial tiles of all slices
+  // (slice z at out + z * M * ldo) and converts them into the result + BN statistics — no separate finalize launch.
   uint32_t* tile_counters;   // [m_tiles * n_tiles], zero at rest (self-resetting)
   void* fin_out;             // activation-typed destination [M][fin_ld]
   long long fin_ld;
@@ -386,15 +386,18 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       } else {
         row_off = static_cast<long long>(row) * p.ldo;
       }
-      // split-K: the K slices of a tile add their partial sums in slice order (blockIdx.z) behind a turn counter, so the
-      // fp32 sums are the same every run; the last slice then owns the finished tile
+      // split-K with in-kernel finalisation (tile_counters): every K slice stores its partial tile into slice z of `out`
+      // ([k_split][M][ldo]); the last slice of the tile to arrive adds the k_split partials in slice order.  Without
+      // tile_counters the slices add into `out` in slice order (blockIdx.z) behind a turn counter.  Either way the fp32
+      // sums are the same every run.
+      const uint32_t tix = blockIdx.x * gridDim.y + blockIdx.y;
       uint32_t* turn = nullptr;
-      if ((p.epi == EPI_F32_ATOMIC || p.epi == EPI_F32_ATOMIC_T) && gridDim.z > 1) {
-        const uint32_t tix = blockIdx.x * gridDim.y + blockIdx.y;
-        turn = p.tile_counters != nullptr ? p.tile_counters + tix : p.det.ctr + DET_TURN_BASE + tix;
+      if ((p.epi == EPI_F32_ATOMIC || p.epi == EPI_F32_ATOMIC_T) && gridDim.z > 1 && p.tile_counters == nullptr) {
+        turn = p.det.ctr + DET_TURN_BASE + tix;
         if (et == 0) turn_wait(turn, blockIdx.z);
         asm volatile("bar.sync 1, 128;" ::: "memory");
       }
+      const long long slice = static_cast<long long>(p.M) * p.ldo;   // floats per partial tile set
 #pragma unroll 1
       for (int c = 0; c < BLOCK_N; c += 32) {
         uint32_t v[32];
@@ -476,7 +479,14 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = static
           }
           if (et == 0 && c == 0) SLB_STAMP(15);
         } else if (p.epi == EPI_F32_ATOMIC) {
-          if (row_store) {
+          if (row_store && p.tile_counters != nullptr) {
+            // conv split-K partial (Nout % 32 == 0: whole, 16-byte aligned 32-column chunks)
+            float4* o4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + blockIdx.z * slice + row_off + col0);
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+              __stcg(o4 + j, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
+                                         __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3])));
+          } else if (row_store) {
             float* o = reinterpret_cast<float*>(p.out) + row_off + col0;
             if (col0 + 32 <= p.N && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
 #pragma unroll
@@ -521,8 +531,14 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = __uint
         if (et == 0) turn_pass(turn, blockIdx.z, gridDim.z);
       }
       if (p.epi == EPI_F32_ATOMIC && p.tile_counters != nullptr) {
-        // ---- serial split-K tail: the last slice of this tile finalises it ----
-        if (et == 0) s_flag[1] = (gridDim.z == 1 || blockIdx.z == gridDim.z - 1) ? 1u : 0u;
+        // ---- split-K tail: the last slice of this tile to arrive sums the partials and finalises the tile ----
+        __threadfence();                                       // this slice's partial is visible before it arrives
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        if (et == 0) {
+          const uint32_t t = atomicAdd(p.tile_counters + tix, 1u);
+          s_flag[1] = (t == gridDim.z - 1u) ? 1u : 0u;
+          if (s_flag[1]) p.tile_counters[tix] = 0;             // zero at rest
+        }
         asm volatile("bar.sync 1, 128;" ::: "memory");
         if (s_flag[1]) {
           __threadfence();
@@ -530,16 +546,22 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = __uint
           for (int c = 0; c < BLOCK_N; c += 32) {
             const int col0 = n0 + c;
             float f[32];
+#pragma unroll
+            for (int j = 0; j < 32; ++j) f[j] = 0.f;
             if (row_ok) {
+              // +0 plus the slices in slice order with add.rn.ftz: the arithmetic of red.global.add.f32 into a zeroed buffer
               const float4* a4 = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.out) + row_off + col0);
+#pragma unroll 1
+              for (int zz = 0; zz < static_cast<int>(gridDim.z); ++zz) {
 #pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float4 t4 = __ldcg(a4 + j);
-                f[4 * j] = t4.x; f[4 * j + 1] = t4.y; f[4 * j + 2] = t4.z; f[4 * j + 3] = t4.w;
+                for (int j = 0; j < 8; ++j) {
+                  const float4 t4 = __ldcg(a4 + zz * (slice / 4) + j);
+                  asm("add.rn.ftz.f32 %0, %0, %1;" : "+f"(f[4 * j]) : "f"(t4.x));
+                  asm("add.rn.ftz.f32 %0, %0, %1;" : "+f"(f[4 * j + 1]) : "f"(t4.y));
+                  asm("add.rn.ftz.f32 %0, %0, %1;" : "+f"(f[4 * j + 2]) : "f"(t4.z));
+                  asm("add.rn.ftz.f32 %0, %0, %1;" : "+f"(f[4 * j + 3]) : "f"(t4.w));
+                }
               }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = 0.f;
             }
 #pragma unroll
             for (int j = 0; j < 32; ++j) f[j] += s_bias[c + j];
@@ -757,52 +779,53 @@ int slb_preload_gemm() {
 // sum / sum-of-squares accumulation (caller zeroes them).  flip=1 computes the input gradient:
 // x := dY [B,H,W,Cout_w], w as stored, out = dX[B,H,W,Cin_w]  (then Cin here means channels of A = Cout_w).
 // dtype: 0 = bf16 tensors (wgmma bf16), 1 = fp32 tensors (wgmma tf32); x, w and y share it.
-// block_n in {64,128,256} (0 = auto); k_split > 1 accumulates fp32 partial sums into `acc` ([M][Nout], zeroed by the
-// caller) with vector red.add instead of writing y — the last K slice of a tile (tile_counters) or slb_conv_finalize
-// then produces y.
+// block_n in {64,128,256} (0 = auto); k_split > 1 with tile_counters: every K slice stores its fp32 partial sums into
+// `acc` ([k_split][M][Nout], acc_cap floats, no zeroing needed) and the last slice of a tile to arrive adds them in slice
+// order and produces y.  Without tile_counters the slices add into `acc` ([M][Nout], zeroed by the caller) with vector
+// red.add in slice order and slb_conv_finalize produces y.
 struct BnbArgs { const void* y; const float *mean, *istd, *gamma, *beta; int relu, pool; };
 struct PubArgs { uint32_t *ticket, *flag, *seq; };
 static int conv_igemm_impl(const void* x, const void* w, void* y, const float* bias, float* col_sum, float* col_sumsq,
                            int B, int H, int W, int Ca, int Nout, int flip, int w_cin, int w_cout, int block_n, int k_split,
-                           float* acc, uint32_t* tile_counters, const BnbArgs* bnb, int dtype, cudaStream_t st,
+                           float* acc, long long acc_cap, uint32_t* tile_counters, const BnbArgs* bnb, int dtype, cudaStream_t st,
                            const PubArgs* pub = nullptr);
 
 // conv / dgrad whose last CTA also publishes a mailbox flag (cut-head dgrad storing dX into the upstream stage's HBM)
 int slb_conv3x3_igemm_pub(const void* x, const void* w, void* y, const float* bias, float* col_sum, float* col_sumsq,
                           int B, int H, int W, int Ca, int Nout, int flip, int w_cin, int w_cout, int block_n, int k_split,
-                          float* acc, uint32_t* tile_counters, int dtype, uint32_t* pub_ticket, uint32_t* pub_flag,
+                          float* acc, long long acc_cap, uint32_t* tile_counters, int dtype, uint32_t* pub_ticket, uint32_t* pub_flag,
                           uint32_t* pub_seq, cudaStream_t st) {
   if (k_split > 1 && tile_counters == nullptr) return -18;      // the flag must follow the *final* dX stores
   PubArgs pa = {pub_ticket, pub_flag, pub_seq};
   return conv_igemm_impl(x, w, y, bias, col_sum, col_sumsq, B, H, W, Ca, Nout, flip, w_cin, w_cout, block_n, k_split, acc,
-                         tile_counters, nullptr, dtype, st, pub_flag != nullptr ? &pa : nullptr);
+                         acc_cap, tile_counters, nullptr, dtype, st, pub_flag != nullptr ? &pa : nullptr);
 }
 
 int slb_conv3x3_igemm(const void* x, const void* w, void* y, const float* bias, float* col_sum, float* col_sumsq,
                       int B, int H, int W, int Ca /*channels of A*/, int Nout /*output channels*/, int flip,
                       int w_cin /*Cin of the weight tensor*/, int w_cout, int block_n, int k_split, float* acc,
-                      uint32_t* tile_counters, int dtype, cudaStream_t st) {
+                      long long acc_cap, uint32_t* tile_counters, int dtype, cudaStream_t st) {
   return conv_igemm_impl(x, w, y, bias, col_sum, col_sumsq, B, H, W, Ca, Nout, flip, w_cin, w_cout, block_n, k_split, acc,
-                         tile_counters, nullptr, dtype, st);
+                         acc_cap, tile_counters, nullptr, dtype, st);
 }
 
 // dgrad whose epilogue also reduces the BatchNorm backward sums of the upstream block: dbeta / dgamma (zeroed by the
 // caller) receive sum m*dX and sum m*dX*xhat; needs k_split == 1 or in-kernel finalisation (tile_counters).  bf16 only.
 int slb_conv3x3_dgrad_bnstats(const void* dy, const void* w, void* dx, int B, int H, int W, int Ca, int Nout, int w_cin,
-                              int w_cout, int block_n, int k_split, float* acc, uint32_t* tile_counters,
+                              int w_cout, int block_n, int k_split, float* acc, long long acc_cap, uint32_t* tile_counters,
                               const void* up_y, const float* up_mean, const float* up_istd, const float* up_gamma,
                               const float* up_beta, int up_relu, int up_pool, float* dbeta, float* dgamma, cudaStream_t st) {
   if (k_split > 1 && tile_counters == nullptr) return -18;
   BnbArgs b = {up_y, up_mean, up_istd, up_gamma, up_beta, up_relu, up_pool};
   return conv_igemm_impl(dy, w, dx, nullptr, dbeta, dgamma, B, H, W, Ca, Nout, 1, w_cin, w_cout, block_n, k_split, acc,
-                         tile_counters, &b, 0, st);
+                         acc_cap, tile_counters, &b, 0, st);
 }
 
 }  // extern "C"
 
 static int conv_igemm_impl(const void* x, const void* w, void* y, const float* bias, float* col_sum, float* col_sumsq,
                            int B, int H, int W, int Ca, int Nout, int flip, int w_cin, int w_cout, int block_n, int k_split,
-                           float* acc, uint32_t* tile_counters, const BnbArgs* bnb, int dtype, cudaStream_t st,
+                           float* acc, long long acc_cap, uint32_t* tile_counters, const BnbArgs* bnb, int dtype, cudaStream_t st,
                            const PubArgs* pub) {
   const int KE = 128 / esize(dtype);
   if (Ca % KE != 0 || Nout % 32 != 0) return -10;
@@ -833,6 +856,8 @@ static int conv_igemm_impl(const void* x, const void* w, void* y, const float* b
   p.a_mn = 0; p.b_mn = flip ? 1 : 0; p.ldo = Nout;
   if (k_split > 1) {
     if (acc == nullptr) return -17;
+    // in-kernel finalisation: k_split partial tile sets [k_split][M][Nout]; otherwise one zeroed [M][Nout] accumulator
+    if (acc_cap < (tile_counters != nullptr ? (long long)k_split : 1LL) * M * Nout) return -19;
     p.epi = EPI_F32_ATOMIC; p.out = acc;
     if (tile_counters != nullptr) {       // in-kernel finalisation by the last K-slice of every tile
       p.tile_counters = tile_counters; p.fin_out = y; p.fin_ld = Nout;

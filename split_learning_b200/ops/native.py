@@ -137,10 +137,21 @@ def _ke(t) -> int:
     return 32 if _dt(t).value == 1 else 64
 
 
+def _cap(acc) -> c_longlong:
+    return c_longlong(0 if acc is None else acc.numel())
+
+
+def conv_partial_floats(M: int, N: int, k_split: int) -> int:
+    """Floats of the split-K partial buffer a conv / dgrad with in-kernel finalisation (``counters``) needs."""
+    return M * N * k_split if k_split > 1 else 0
+
+
 def conv3x3_fwd(x, w_bf16, y, bias=None, col_sum=None, col_sumsq=None, acc=None, tiling=None, counters=None):
     """x [B,H,W,Cin], w [Cout,3,3,Cin] -> y [B,H,W,Cout] (pre-BN) + optional BN sums; x / w / y all bf16 (wgmma bf16)
-    or all fp32 (wgmma tf32).  ``acc``: zeroed fp32 [M, Cout] scratch enabling split-K (the last K slice of a tile —
-    or a finalize kernel — then produces y and the sums)."""
+    or all fp32 (wgmma tf32).  ``acc`` enables split-K.  With ``counters`` it is an fp32 buffer of at least
+    ``conv_partial_floats(M, Cout, k_split)`` floats (no zeroing needed): every K slice stores its partial tiles there and
+    the last slice of a tile to arrive adds them in slice order and produces y and the sums.  Without ``counters`` it is a
+    zeroed fp32 [M, Cout] accumulator and a finalize kernel produces y."""
     B, H, W, Cin = x.shape
     Cout = w_bf16.shape[0]
     bn, ks = tiling or conv_tiling(B * H * W, Cout, Cin, ke=_ke(x))
@@ -148,7 +159,7 @@ def conv3x3_fwd(x, w_bf16, y, bias=None, col_sum=None, col_sumsq=None, acc=None,
         ks = 1
     _check(lib().slb_conv3x3_igemm(_p(x), _p(w_bf16), _p(y), _p(bias), _p(col_sum), _p(col_sumsq), c_int(B), c_int(H),
                                    c_int(W), c_int(Cin), c_int(Cout), c_int(0), c_int(Cin), c_int(Cout), c_int(bn), c_int(ks),
-                                   _p(acc), _p(counters), _dt(x), _stream()), "conv3x3_fwd")
+                                   _p(acc), _cap(acc), _p(counters), _dt(x), _stream()), "conv3x3_fwd")
     if ks > 1 and counters is None:
         conv_finalize(acc, bias, y, col_sum, col_sumsq)
 
@@ -169,7 +180,7 @@ def conv3x3_dgrad(dy, w_bf16, dx, acc=None, tiling=None, counters=None, bn_stats
             raise NativeError("conv3x3_dgrad(bn_stats=) needs in-kernel split-K finalisation (counters)")
         uy, mean, istd, gamma, beta, relu, pool, dgamma, dbeta = bn_stats
         _check(lib().slb_conv3x3_dgrad_bnstats(_p(dy), _p(w_bf16), _p(dx), c_int(B), c_int(H), c_int(W), c_int(Cout), c_int(Cin),
-                                               c_int(Cin), c_int(Cout), c_int(bn), c_int(ks), _p(acc), _p(counters), _p(uy),
+                                               c_int(Cin), c_int(Cout), c_int(bn), c_int(ks), _p(acc), _cap(acc), _p(counters), _p(uy),
                                                _p(mean), _p(istd), _p(gamma), _p(beta), c_int(int(relu)), c_int(int(pool)), _p(dbeta), _p(dgamma),
                                                _stream()), "conv3x3_dgrad_bnstats")
         return
@@ -178,12 +189,12 @@ def conv3x3_dgrad(dy, w_bf16, dx, acc=None, tiling=None, counters=None, bn_stats
         ticket, flag, seq = publish
         _check(lib().slb_conv3x3_igemm_pub(_p(dy), _p(w_bf16), _p(dx), _p(None), _p(None), _p(None), c_int(B), c_int(H), c_int(W),
                                            c_int(Cout), c_int(Cin), c_int(1), c_int(Cin), c_int(Cout), c_int(bn), c_int(ks),
-                                           _p(acc), _p(counters), _dt(dy), _p(ticket), _p(flag), _p(seq), _stream()),
+                                           _p(acc), _cap(acc), _p(counters), _dt(dy), _p(ticket), _p(flag), _p(seq), _stream()),
                "conv3x3_dgrad_pub")
         return
     _check(lib().slb_conv3x3_igemm(_p(dy), _p(w_bf16), _p(dx), _p(None), _p(None), _p(None), c_int(B), c_int(H), c_int(W),
                                    c_int(Cout), c_int(Cin), c_int(1), c_int(Cin), c_int(Cout), c_int(bn), c_int(ks), _p(acc),
-                                   _p(counters), _dt(dy), _stream()), "conv3x3_dgrad")
+                                   _cap(acc), _p(counters), _dt(dy), _stream()), "conv3x3_dgrad")
     if ks > 1 and counters is None:
         conv_finalize(acc, None, dx, None, None)
 
@@ -345,17 +356,27 @@ def conv3x3_small_wgrad(x_nchw_f32, dy, dw_f32):
                                          c_int(Cout), _dt(dy), _stream()), "conv3x3_small_wgrad")
 
 
+def _slices(acc):
+    """(parts, B, N) of a Linear result: a contiguous fp32 [parts, B, N] stack of slice partials (linear_fwd_f32 /
+    linear_dgrad_f32), which the consumer adds in slice order, or a finished [B, N] buffer (parts = 0)."""
+    if acc.dim() == 3:
+        if acc.dtype != torch.float32 or not acc.is_contiguous():
+            raise NativeError("slice partials must be a contiguous fp32 [parts, B, N] stack")
+        return tuple(acc.shape)
+    return (0,) + tuple(acc.shape)
+
+
 def linear_finalize(acc, bias, out_bf16, out_f32, mask, relu, drop_p=0.0, seed=0, step_ptr=None):
-    B, N = acc.shape
+    parts, B, N = _slices(acc)
     ldo = out_bf16.stride(0) if out_bf16 is not None else N
-    _check(lib().slb_linear_finalize(_p(acc), _p(bias), _p(out_bf16), _p(out_f32), _p(mask), c_int(B), c_int(N), c_int(ldo),
-                                     c_int(int(relu)), c_float(drop_p), c_uint32(seed), _p(step_ptr),
+    _check(lib().slb_linear_finalize(_p(acc), c_int(parts), _p(bias), _p(out_bf16), _p(out_f32), _p(mask), c_int(B), c_int(N),
+                                     c_int(ldo), c_int(int(relu)), c_float(drop_p), c_uint32(seed), _p(step_ptr),
                                      _dt(out_bf16) if out_bf16 is not None else c_int(0), _stream()), "linear_finalize")
 
 
 def linear_bwd_prep(dacc, yout, mask, dz, dbias, relu, drop_p=0.0):
-    B, N = dacc.shape
-    _check(lib().slb_linear_bwd_prep(_p(dacc), _p(yout), _p(mask), _p(dz), _p(dbias), c_int(B), c_int(N),
+    parts, B, N = _slices(dacc)
+    _check(lib().slb_linear_bwd_prep(_p(dacc), c_int(parts), _p(yout), _p(mask), _p(dz), _p(dbias), c_int(B), c_int(N),
                                      c_int(yout.stride(0) if yout is not None else N), c_int(dz.stride(0)),
                                      c_int(int(relu)), c_float(drop_p), _dt(dz), _stream()), "linear_bwd_prep")
 
@@ -366,24 +387,50 @@ def dropout_fwd(x, y, mask, p, seed, step_ptr=None):
 
 
 def dropout_bwd(dacc, mask, dx, p):
-    _check(lib().slb_dropout_bwd(_p(dacc), _p(mask), _p(dx), c_longlong(dacc.numel()), c_float(p), _dt(dx), _stream()),
+    """dx = dropout backward of dacc (mask None: a plain copy / cast; a stack of slice partials is summed first)."""
+    parts = _slices(dacc)[0] if dacc.dim() == 3 else 0
+    n = dacc.numel() // max(parts, 1)
+    _check(lib().slb_dropout_bwd(_p(dacc), c_int(parts), _p(mask), _p(dx), c_longlong(n), c_float(p), _dt(dx), _stream()),
            "dropout_bwd")
 
 
 # ---- fp32 Linear on the CUDA cores (parity mode: the reference's nn.Linear is a plain fp32 GEMM)
-def linear_fwd_f32(x, w, acc):
-    """acc[b][out] (fp32, zeroed) += x[b][in] @ w[out][in]^T, IEEE fp32 FMAs."""
+def linear_f32_slices(dgrad: bool, out_f: int, in_f: int) -> int:
+    """Number of slice partials linear_fwd_f32 (dgrad False) or linear_dgrad_f32 (True) writes for this weight shape."""
+    s = lib().slb_linear_f32_slices(c_int(int(dgrad)), c_int(out_f), c_int(in_f))
+    if s < 1:
+        raise NativeError(f"linear_f32_slices: bad shape {out_f}x{in_f}")
+    return s
+
+
+def _part_view(part, S, Bn, n):
+    if part.dtype != torch.float32 or not part.is_contiguous():
+        raise NativeError("partial buffer must be contiguous fp32")
+    if part.numel() < S * Bn * n:
+        raise NativeError(f"partial buffer too small: {part.numel()} floats < {S} slices x {Bn} x {n}")
+    return part.reshape(-1)[:S * Bn * n].view(S, Bn, n)
+
+
+def linear_fwd_f32(x, w, part):
+    """Slice partials of x[b][in] @ w[out][in]^T in IEEE fp32 FMAs, stored into the fp32 buffer ``part`` (no zeroing
+    needed).  Returns the [slices, B, out] view of ``part`` that linear_finalize (or dropout_bwd) adds up in slice order."""
     Bn, K = x.shape
-    _check(lib().slb_linear_fwd_f32(_p(x), _p(w), _p(acc), c_int(Bn), c_int(w.shape[0]), c_int(K), c_int(x.stride(0)),
-                                    c_int(w.stride(0)), c_int(acc.stride(0)), _stream()), "linear_fwd_f32")
+    out_f = w.shape[0]
+    pv = _part_view(part, linear_f32_slices(False, out_f, K), Bn, out_f)
+    _check(lib().slb_linear_fwd_f32(_p(x), _p(w), _p(part), c_longlong(part.numel()), c_int(Bn), c_int(out_f), c_int(K),
+                                    c_int(x.stride(0)), c_int(w.stride(0)), _stream()), "linear_fwd_f32")
+    return pv
 
 
-def linear_dgrad_f32(dz, w, dacc):
-    """dacc[b][in] (fp32, zeroed) += dz[b][out] @ w[out][in]."""
+def linear_dgrad_f32(dz, w, part):
+    """Slice partials of dz[b][out] @ w[out][in] into ``part``; returns the [slices, B, in] view that linear_bwd_prep or
+    dropout_bwd adds up in slice order."""
     Bn = dz.shape[0]
     out_f, in_f = w.shape
-    _check(lib().slb_linear_dgrad_f32(_p(dz), _p(w), _p(dacc), c_int(Bn), c_int(out_f), c_int(in_f), c_int(dz.stride(0)),
-                                      c_int(w.stride(0)), c_int(dacc.stride(0)), _stream()), "linear_dgrad_f32")
+    pv = _part_view(part, linear_f32_slices(True, out_f, in_f), Bn, in_f)
+    _check(lib().slb_linear_dgrad_f32(_p(dz), _p(w), _p(part), c_longlong(part.numel()), c_int(Bn), c_int(out_f), c_int(in_f),
+                                      c_int(dz.stride(0)), c_int(w.stride(0)), _stream()), "linear_dgrad_f32")
+    return pv
 
 
 def linear_wgrad_f32(dz, x, g=None, sgd=None, accumulate=False):

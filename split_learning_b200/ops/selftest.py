@@ -86,7 +86,7 @@ def _conv_fwd(dt):
         s1 = torch.zeros(Cout, device="cuda")
         s2 = torch.zeros(Cout, device="cuda")
         bn_, ks_ = N.conv_tiling(B * H * W, Cout, Cin, ke=32 if dt == F32 else 64)
-        acc = torch.zeros(B * H * W, Cout, device="cuda") if ks_ > 1 else None
+        acc = torch.zeros(N.conv_partial_floats(B * H * W, Cout, ks_), device="cuda") if ks_ > 1 else None   # partials
         ctr = torch.zeros(4096, device="cuda", dtype=torch.int32)
         N.conv3x3_fwd(x, w, y, bias, s1, s2, acc=acc, counters=ctr)          # in-kernel split-K finalisation
         if ks_ > 1:                                                           # ... and the two-kernel variant
@@ -129,7 +129,7 @@ def _conv_dgrad(dt):
         dy = torch.randn(B, H, W, Cout, device="cuda").to(dt)
         dx = torch.empty(B, H, W, Cin, device="cuda", dtype=dt)
         bn_, ks_ = N.conv_tiling(B * H * W, Cin, Cout, flip=1, ke=32 if dt == F32 else 64)
-        acc = torch.zeros(B * H * W, Cin, device="cuda") if ks_ > 1 else None
+        acc = torch.zeros(N.conv_partial_floats(B * H * W, Cin, ks_), device="cuda") if ks_ > 1 else None
         ctr = torch.zeros(4096, device="cuda", dtype=torch.int32)       # must outlive the asynchronous kernel
         N.conv3x3_dgrad(dy, w, dx, acc=acc, counters=ctr)
         torch.cuda.synchronize()
@@ -168,7 +168,7 @@ def conv_dgrad_bn_stats():
             gamma = torch.rand(Cin, device="cuda") + 0.5
             beta = torch.randn(Cin, device="cuda") * 0.3
             bn_, ks_ = N.conv_tiling(B * H * W, Cin, Cout, flip=1)
-            acc = torch.zeros(B * H * W, Cin, device="cuda") if ks_ > 1 else None
+            acc = torch.zeros(N.conv_partial_floats(B * H * W, Cin, ks_), device="cuda") if ks_ > 1 else None
             ctr = torch.zeros(4096, device="cuda", dtype=torch.int32)
             dx = torch.empty(B, H, W, Cin, device="cuda", dtype=torch.bfloat16)
             dgamma, dbeta = torch.zeros(Cin, device="cuda"), torch.zeros(Cin, device="cuda")
@@ -227,16 +227,18 @@ def linear_f32():
         torch.manual_seed(7)
         x = torch.randn(Bn, inf, device="cuda")
         w = torch.randn(outf, inf, device="cuda") / inf ** 0.5
-        acc = torch.zeros(Bn, outf, device="cuda")
-        N.linear_fwd_f32(x, w, acc)
+        part = torch.full((N.linear_f32_slices(False, outf, inf) * Bn * outf,), float("nan"), device="cuda")
+        acc = torch.empty(Bn, outf, device="cuda")
+        N.dropout_bwd(N.linear_fwd_f32(x, w, part), None, acc, 0.0)        # slice partials summed in slice order
         torch.cuda.synchronize()
         e1 = _rel(acc, x @ w.t())
         ld = pad or outf
         dzp = torch.zeros(Bn, ld, device="cuda")
         dzp[:, :outf] = torch.randn(Bn, outf, device="cuda")
         dz = dzp[:, :outf]
-        dacc = torch.zeros(Bn, inf, device="cuda")
-        N.linear_dgrad_f32(dz, w, dacc)
+        part = torch.full((N.linear_f32_slices(True, outf, inf) * Bn * inf,), float("nan"), device="cuda")
+        dacc = torch.empty(Bn, inf, device="cuda")
+        N.dropout_bwd(N.linear_dgrad_f32(dz, w, part), None, dacc, 0.0)
         torch.cuda.synchronize()
         e2 = _rel(dacc, dz @ w)
         dw = torch.full((outf, inf), 7.0, device="cuda")

@@ -536,9 +536,16 @@ class _Plan:
         else:
             self.x_in = [torch.zeros(B, ex.in_shape[0], device=dev, dtype=bf) for _ in range(self.n_slots)]
         self.labels = torch.zeros(B, device=dev, dtype=torch.int64)
-        # ---- zero-scratch (BN sums, fp32 GEMM accumulators): one contiguous region, one zero kernel per pass
+        # ---- zero-scratch (BN sums, split-K accumulators of the bf16 Linear GEMMs): one contiguous region, one zero kernel
+        # per pass
         scratch = 0
         self.soff: Dict[Tuple[int, str], Tuple[int, int]] = {}
+        # ---- split-K / slice partials of the conv kernels (in-kernel finalisation) and the fp32 Linear kernels: every
+        # element is stored before it is read, so they need no zeroing.  One region serves every such launch of the plan:
+        # all of them run on the plan's stream, a conv launch adds up its own partials before it completes, and the kernel
+        # that adds up a Linear launch's partials (linear_finalize / linear_bwd_prep / dropout_bwd) precedes the next
+        # launch that writes the region.
+        part = 0
 
         def reserve(key, n):
             nonlocal scratch
@@ -551,15 +558,19 @@ class _Plan:
                     reserve((bi, "sumsq"), b.cout)
                 if b.conv is not None and b.cin > 4:
                     M = B * b.H * b.W
-                    if N.conv_tiling(M, b.cout, b.cin, ke=self.ke)[1] > 1:
-                        reserve((bi, "facc"), M * b.cout)           # split-K partial sums, forward
-                    if train and N.conv_tiling(M, b.cin, b.cout, flip=1, ke=ex.ke)[1] > 1 and not (bi == 0 and ex.is_first):
-                        reserve((bi, "dacc"), M * b.cin)            # split-K partial sums, dgrad
+                    part = max(part, N.conv_partial_floats(M, b.cout, N.conv_tiling(M, b.cout, b.cin, ke=self.ke)[1]))
+                    if train and not (bi == 0 and ex.is_first):
+                        part = max(part, N.conv_partial_floats(M, b.cin, N.conv_tiling(M, b.cin, b.cout, flip=1, ke=ex.ke)[1]))
+            elif isinstance(b, LinearBlock) and self.fp32:
+                part = max(part, N.linear_f32_slices(False, b.fout, b.fin) * B * b.fout)
+                if train:
+                    part = max(part, N.linear_f32_slices(True, b.fout, b.fin) * B * b.fin)
             elif isinstance(b, LinearBlock):
                 reserve((bi, "acc"), B * b.fout)
                 if train:
                     reserve((bi, "dacc_in"), B * b.fin)
         self.scratch = torch.zeros(max(scratch, 4), device=dev)
+        self.part = torch.zeros(part, device=dev) if part else None
         # ---- activations
         self.act: List[Dict[str, torch.Tensor]] = []
         for bi, b in enumerate(ex.blocks):
@@ -658,7 +669,7 @@ class _Plan:
                 plain = b.conv is not None and b.bn is None          # cut right after the conv (e.g. cut 4)
                 if plain:
                     tgt = a["y"] if not (is_final and out_ptr_override is not None) else out_ptr_override
-                    facc = self.s(bi, "facc") if (bi, "facc") in self.soff else None
+                    facc = self.part
                     N.conv3x3_fwd(x, self.W(f"layer{b.conv}.weight"), tgt, ex.view(ex.P, f"layer{b.conv}.bias"),
                                   acc=facc, counters=self.tile_counters)
                     if is_final and publish is not None:
@@ -694,7 +705,7 @@ class _Plan:
                     if b.cin <= 4:
                         N.conv3x3_small_fwd(x, ex.view(ex.P, f"layer{b.conv}.weight"), bias, a["y"], s1, s2)
                     else:
-                        facc = self.s(bi, "facc") if (bi, "facc") in self.soff else None
+                        facc = self.part
                         N.conv3x3_fwd(x, self.W(f"layer{b.conv}.weight"), a["y"], bias, s1, s2, acc=facc,
                                       counters=self.tile_counters)
                     y = a["y"]
@@ -733,11 +744,11 @@ class _Plan:
             else:
                 xin = x.reshape(self.B, -1)
                 a["in"] = xin
-                acc = self.s(bi, "acc", (self.B, b.fout))
                 w = self.W(f"layer{b.lin}.weight")
                 if self.fp32:
-                    N.linear_fwd_f32(xin, w, acc)
+                    acc = N.linear_fwd_f32(xin, w, self.part)      # slice partials, summed by linear_finalize
                 else:
+                    acc = self.s(bi, "acc", (self.B, b.fout))
                     N.linear_fwd(xin, w, acc, k_split=max(1, min(8, (b.fin // 64) // 8)))
                 if ev:
                     N.linear_finalize(acc, ex.view(ex.P, f"layer{b.lin}.bias"),
@@ -792,10 +803,10 @@ class _Plan:
                 elif not fuse_sgd:
                     on_side(lambda a=a, wkey=wkey: N.linear_wgrad_f32(a["dz"], a["in"], g=ex.view(ex.G, wkey)))
                 if need_dx:
-                    dacc = self.s(bi, "dacc_in", (self.B, b.fin))
-                    if ex.fp32:
-                        N.linear_dgrad_f32(a["dz"], ex.W(wkey), dacc)
+                    if ex.fp32:                                     # slice partials, summed by the consumer of g
+                        dacc = N.linear_dgrad_f32(a["dz"], ex.W(wkey), self.part)
                     else:
+                        dacc = self.s(bi, "dacc_in", (self.B, b.fin))
                         N.linear_dgrad(a["dz"], ex.W(wkey), dacc, k_split=max(1, min(8, (b.fout // 64) // 8)))
                     g = dacc
                     if bi == 0:                                     # stage input gradient leaves in the activation dtype
@@ -813,7 +824,7 @@ class _Plan:
                 N.dropout_bwd(g, a["mask"], a["dx"], b.p)
                 g = a["dx"]
             else:
-                if g.dtype != ex.act_dtype:                         # fp32 accumulator of a Linear block into a bf16 conv block
+                if g.dim() == 3 or g.dtype != ex.act_dtype:         # a Linear block's fp32 slice partials / bf16-mode accumulator
                     tmp = a["dout_bf16"]
                     N.dropout_bwd(g, None, tmp, 0.0)
                     g = tmp
@@ -846,7 +857,7 @@ class _Plan:
                         on_side(lambda a=a, b=b, dy=dy: N.conv3x3_wgrad(a["in"], dy, ex.view(ex.G, f"layer{b.conv}.weight")))
                         if need_dx:
                             dx = a["dx"] if not (bi == 0 and grad_out_override is not None) else grad_out_override
-                            dacc = self.s(bi, "dacc") if (bi, "dacc") in self.soff else None
+                            dacc = self.part
                             stats = None
                             up = ex.blocks[bi - 1] if bi > 0 else None
                             if (ex.fused_bn_stats and not ex.fp32 and isinstance(up, ConvBlock) and up.conv is not None and up.bn is not None

@@ -27,7 +27,7 @@ def main():
         w = (torch.randn(Cout, 3, 3, Cin, device="cuda") * 0.05).to(dt)
         bias = torch.zeros(Cout, device="cuda")
         out = torch.empty(B, HW, HW, Cout, device="cuda", dtype=dt)
-        acc = torch.zeros(M, Cout, device="cuda")
+        acc = torch.zeros(N.conv_partial_floats(M, Cout, max(k for _, k in CONFIGS)), device="cuda")
         s1, s2 = torch.zeros(Cout, device="cuda"), torch.zeros(Cout, device="cuda")
         for (bn, ks) in CONFIGS:
             if Cout % bn:

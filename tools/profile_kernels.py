@@ -92,9 +92,10 @@ def _conv_fwd(B, H, W, Cin, Cout, iters):
     x, w, bias = conv_case(B, H, W, Cin, Cout)
     y = torch.empty(B, H, W, Cout, device="cuda", dtype=ADT())
     s1, s2 = torch.zeros(Cout, device="cuda"), torch.zeros(Cout, device="cuda")
-    bn_, ks = N.conv_tiling(B * H * W, Cout, Cin)
-    acc = torch.zeros(B * H * W, Cout, device="cuda") if ks > 1 else None
-    med, best = timeit(lambda: N.conv3x3_fwd(x, w, y, bias, s1, s2, acc=acc), iters, (lambda: acc.zero_()) if acc is not None else None)
+    bn_, ks = N.conv_tiling(B * H * W, Cout, Cin, ke=32 if PREC == "tf32" else 64)      # the executor's tiling
+    acc = torch.empty(N.conv_partial_floats(B * H * W, Cout, ks), device="cuda") if ks > 1 else None
+    ctr = torch.zeros(4096, device="cuda", dtype=torch.int32)
+    med, best = timeit(lambda: N.conv3x3_fwd(x, w, y, bias, s1, s2, acc=acc, counters=ctr), iters)
     flops = 2.0 * B * H * W * Cout * 9 * Cin
     byts = (x.numel() + w.numel() + y.numel()) * ISZ()
     return {"us": med, "best_us": best, "flops": flops, "bytes": byts, "tiling": [bn_, ks]}
@@ -203,23 +204,50 @@ def fused_cut7_b128(iters):
     return _fused(128, 32, 32, 64, 64, 1, 1, iters)
 
 
-@case
-def linear50_fwd_f32(iters):
-    """fp32 Linear 4096 -> 4096 at batch 32 (parity mode): IEEE fp32 FMAs on CUDA cores, weight streamed once."""
-    x = torch.randn(32, 4096, device="cuda")
-    w = torch.randn(4096, 4096, device="cuda") * 0.01
-    acc = torch.zeros(32, 4096, device="cuda")
-    med, best = timeit(lambda: N.linear_fwd_f32(x, w, acc), iters, lambda: acc.zero_())
-    return {"us": med, "best_us": best, "flops": 2.0 * 32 * 4096 * 4096, "bytes": w.numel() * 4 + x.numel() * 4 + acc.numel() * 4, "fp32_cuda_cores": True}
+def _linear_f32(dgrad, fin, fout, iters):
+    """fp32 Linear at batch 32 (parity mode) as the executor runs it: the sliced kernel storing its partials, then the
+    consumer adding them in slice order (linear_finalize for the forward, linear_bwd_prep for the input gradient)."""
+    B = 32
+    w = torch.randn(fout, fin, device="cuda") * 0.01
+    slices = N.linear_f32_slices(dgrad, fout, fin)
+    n_out = fin if dgrad else fout
+    part = torch.empty(slices * B * n_out, device="cuda")
+    if dgrad:
+        dz = torch.randn(B, fout, device="cuda")
+        y, g, db = torch.randn(B, fin, device="cuda"), torch.empty(B, fin, device="cuda"), torch.empty(fin, device="cuda")
+        fn = lambda: N.linear_bwd_prep(N.linear_dgrad_f32(dz, w, part), y, None, g, db, True)
+    else:
+        x = torch.randn(B, fin, device="cuda")
+        bias, out = torch.randn(fout, device="cuda"), torch.empty(B, fout, device="cuda")
+        fn = lambda: N.linear_finalize(N.linear_fwd_f32(x, w, part), bias, out, None, None, True)
+    med, best = timeit(fn, iters)
+    return {"us": med, "best_us": best, "flops": 2.0 * B * fin * fout, "bytes": w.numel() * 4 + 2 * part.numel() * 4,
+            "slices": slices, "fp32_cuda_cores": True}
 
 
 @case
-def linear50_dgrad_f32(iters):
-    dz = torch.randn(32, 4096, device="cuda")
-    w = torch.randn(4096, 4096, device="cuda") * 0.01
-    dacc = torch.zeros(32, 4096, device="cuda")
-    med, best = timeit(lambda: N.linear_dgrad_f32(dz, w, dacc), iters, lambda: dacc.zero_())
-    return {"us": med, "best_us": best, "flops": 2.0 * 32 * 4096 * 4096, "bytes": w.numel() * 4 + dz.numel() * 4 + dacc.numel() * 4, "fp32_cuda_cores": True}
+def linear_fwd_f32_512x4096(iters):
+    return _linear_f32(False, 512, 4096, iters)
+
+
+@case
+def linear_fwd_f32_4096x4096(iters):
+    return _linear_f32(False, 4096, 4096, iters)
+
+
+@case
+def linear_fwd_f32_4096x10(iters):
+    return _linear_f32(False, 4096, 10, iters)
+
+
+@case
+def linear_dgrad_f32_4096x4096(iters):
+    return _linear_f32(True, 4096, 4096, iters)
+
+
+@case
+def linear_dgrad_f32_512x4096(iters):
+    return _linear_f32(True, 512, 4096, iters)
 
 
 @case

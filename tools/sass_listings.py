@@ -23,8 +23,8 @@ KERNELS = {
     "sgd_momentum": "_ZN3slb19sgd_momentum_kernelEP6float4S1_S1_P5uint2xffi",
     "attn_fwd": "_ZN3slb15attn_fwd_kernelE14CUtensorMap_stS0_S0_NS_10AttnParamsE",
     "attn_bwd": "_ZN3slb15attn_bwd_kernelE14CUtensorMap_stS0_S0_S0_NS_10AttnParamsE",
-    "linear_fwd_f32_ldgsts": "_ZN3slb21linear_fwd_f32_kernelEPKfS1_Pfiiiiiii",
-    "linear_dgrad_f32_ldgsts": "_ZN3slb23linear_dgrad_f32_kernelEPKfS1_Pfiiiiiii",
+    "linear_fwd_f32_ldgsts": "_ZN3slb21linear_fwd_f32_kernelEPKfS1_Pfiiiiii",
+    "linear_dgrad_f32_ldgsts": "_ZN3slb23linear_dgrad_f32_kernelEPKfS1_Pfiiiiii",
     "ticket_publish": "_ZN3slb21ticket_publish_kernelEPjijjPKjj",
     "ticket_claim": "_ZN3slb19ticket_claim_kernelEPjijyPVj",
     "zero_wait_flag_acquire": "_ZN3slb16zero_wait_kernelEP6float4xPKjPjyPi",
