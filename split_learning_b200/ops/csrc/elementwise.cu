@@ -237,7 +237,9 @@ struct BnFwdParams {
 
 // INFER: BatchNorm in inference mode (module.eval()): scale / shift from running_mean / running_var, no batch statistics
 // and no writes to the running statistics, num_batches_tracked or save_*.
-template <typename T, bool INFER = false>
+// ODD: MaxPool2 over a map with odd H or W (nn.MaxPool2d(2) floor semantics: the last row / column is dropped, the
+// output is floor(H/2) x floor(W/2)).  A separate instantiation, so the even-size kernels keep their code.
+template <typename T, bool INFER = false, bool ODD = false>
 __global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const BnFwdParams<T> p) {
   pdl_trigger();
   pdl_wait();
@@ -276,7 +278,8 @@ __global__ void __launch_bounds__(256) bn_relu_pool_fwd_kernel(const BnFwdParams
 
   const int cg = p.C >> 3;                                  // 8-channel groups
   const int OW = p.pool ? p.W >> 1 : p.W, OH = p.pool ? p.H >> 1 : p.H;
-  const long long outP = p.pool ? static_cast<long long>(p.P) >> 2 : p.P;
+  const long long outP = ODD ? static_cast<long long>(p.P / (p.H * p.W)) * OH * OW
+                              : (p.pool ? static_cast<long long>(p.P) >> 2 : p.P);
   const long long total = outP * cg;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int g = static_cast<int>(i % cg);
@@ -379,8 +382,62 @@ __device__ __forceinline__ void bn_dz(const BnBwdParams<T>& p, long long op, int
   }
 }
 
+// Odd H or W with MaxPool2 (the ODD kernels): position `op` walks the ceil(H/2) x ceil(W/2) grid, so that every pre-pool
+// pixel belongs to exactly one position.  A window on the dropped last row or column has no pooled output: its dz is zero,
+// but its dy is not (the BatchNorm-backward mean terms), so the apply passes still write it.  ip[q] = -1: no pixel.
+template <typename T>
+__device__ __forceinline__ void bn_dz_odd(const BnBwdParams<T>& p, long long op, int g, const float (&sc)[8], const float (&sh)[8],
+                                          float (&yv)[4][8], float (&dz)[4][8], long long (&ip)[4]) {
+  const int OW = p.W >> 1, OH = p.H >> 1, CW = (p.W + 1) >> 1, CH = (p.H + 1) >> 1;
+  const int ow = static_cast<int>(op % CW);
+  const long long t = op / CW;
+  const int oh = static_cast<int>(t % CH);
+  const long long b = t / CH;
+  const bool pooled = ow < OW && oh < OH;
+  float d[8];
+  if (pooled) {
+    load8(p.dout + ((b * OH + oh) * OW + ow) * p.C + g * 8, d);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) d[j] = 0.f;
+  }
+  const long long base = ((b * p.H + 2 * oh) * p.W + 2 * ow);
+  float best[8];
+  int arg[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) { best[j] = -INFINITY; arg[j] = 0; }
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const bool in = 2 * oh + (q >> 1) < p.H && 2 * ow + (q & 1) < p.W;
+    ip[q] = in ? base + (q >> 1) * p.W + (q & 1) : -1;
+    if (in) {
+      load8(p.y + ip[q] * p.C + g * 8, yv[q]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) yv[q][j] = 0.f;
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float z = fmaf(yv[q][j], sc[j], sh[j]);
+      if (p.relu) z = fmaxf(z, 0.f);
+      if (in && z > best[j]) { best[j] = z; arg[j] = q; }   // first maximum wins, like torch
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) dz[q][j] = (pooled && arg[j] == q && !(p.relu && best[j] <= 0.f)) ? d[j] : 0.f;
+}
+
+// positions walked by the backward kernels: pooled windows, or (ODD) the ceil grid of bn_dz_odd
+template <bool POOL, bool ODD, typename T>
+__device__ __forceinline__ long long bn_bwd_positions(const BnBwdParams<T>& p) {
+  if constexpr (ODD) return static_cast<long long>(p.P / (p.H * p.W)) * ((p.H + 1) >> 1) * ((p.W + 1) >> 1);
+  else return POOL ? static_cast<long long>(p.P) >> 2 : p.P;
+}
+
 // pass 1: dgamma / dbeta.  blockDim = (C/8, 256/(C/8)); grid-stride over output positions.
-template <bool POOL, typename T>
+template <bool POOL, typename T, bool ODD = false>
 __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const BnBwdParams<T> p) {
   pdl_trigger();
   pdl_wait();
@@ -396,11 +453,12 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const BnBwdParams<T>
     sh[j] = p.beta[c] - mean[j] * sc[j];
     ag[j] = ab[j] = 0.f;
   }
-  const long long outP = POOL ? static_cast<long long>(p.P) >> 2 : p.P;
+  const long long outP = bn_bwd_positions<POOL, ODD>(p);
   for (long long op = blockIdx.x * (long long)blockDim.y + threadIdx.y; op < outP; op += (long long)gridDim.x * blockDim.y) {
     float yv[NP][8], dz[NP][8];
     long long ip[NP];
-    bn_dz<POOL, T>(p, op, g, sc, sh, yv, dz, ip);
+    if constexpr (ODD) bn_dz_odd<T>(p, op, g, sc, sh, yv, dz, ip);
+    else bn_dz<POOL, T>(p, op, g, sc, sh, yv, dz, ip);
 #pragma unroll
     for (int q = 0; q < NP; ++q)
 #pragma unroll
@@ -427,7 +485,7 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const BnBwdParams<T>
 }
 
 // pass 2: dy = gamma*invstd*(dz - dbeta/P - xhat*dgamma/P)
-template <bool POOL, typename T>
+template <bool POOL, typename T, bool ODD = false>
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const BnBwdParams<T> p) {
   pdl_trigger();
   pdl_wait();
@@ -446,13 +504,15 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const BnBwdParams<T> 
     k1[j] = p.dbeta[c] * invP;
     k2[j] = p.dgamma[c] * invP;
   }
-  const long long outP = POOL ? static_cast<long long>(p.P) >> 2 : p.P;
+  const long long outP = bn_bwd_positions<POOL, ODD>(p);
   for (long long op = blockIdx.x * (long long)blockDim.y + threadIdx.y; op < outP; op += (long long)gridDim.x * blockDim.y) {
     float yv[NP][8], dz[NP][8];
     long long ip[NP];
-    bn_dz<POOL, T>(p, op, g, sc, sh, yv, dz, ip);
+    if constexpr (ODD) bn_dz_odd<T>(p, op, g, sc, sh, yv, dz, ip);
+    else bn_dz<POOL, T>(p, op, g, sc, sh, yv, dz, ip);
 #pragma unroll
     for (int q = 0; q < NP; ++q) {
+      if constexpr (ODD) { if (ip[q] < 0) continue; }
       float r[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -469,7 +529,7 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const BnBwdParams<T> 
 // cross-block reduction at all: pass 1 (dgamma, dbeta) -> block reduction -> pass 2 (dy), one launch instead of the
 // reduce + apply pair (whose second kernel re-reads what the first just read, after a kernel boundary).  The re-read of
 // pass 2 hits L1/L2.  Threads read 32-byte sectors (8 fp32 channels) — full sector efficiency.
-template <bool POOL, typename T>
+template <bool POOL, typename T, bool ODD = false>
 __global__ void __launch_bounds__(256) bn_bwd_chan_kernel(const BnBwdParams<T> p) {
   pdl_trigger();
   pdl_wait();
@@ -485,11 +545,12 @@ __global__ void __launch_bounds__(256) bn_bwd_chan_kernel(const BnBwdParams<T> p
     sh[j] = p.beta[c] - mean[j] * sc[j];
     ag[j] = ab[j] = 0.f;
   }
-  const int outP = POOL ? p.P >> 2 : p.P;
+  const int outP = ODD ? static_cast<int>(bn_bwd_positions<POOL, ODD>(p)) : (POOL ? p.P >> 2 : p.P);
   for (int op = threadIdx.x; op < outP; op += blockDim.x) {
     float yv[NP][8], dz[NP][8];
     long long ip[NP];
-    bn_dz<POOL, T>(p, op, g, sc, sh, yv, dz, ip);
+    if constexpr (ODD) bn_dz_odd<T>(p, op, g, sc, sh, yv, dz, ip);
+    else bn_dz<POOL, T>(p, op, g, sc, sh, yv, dz, ip);
 #pragma unroll
     for (int q = 0; q < NP; ++q)
 #pragma unroll
@@ -529,9 +590,11 @@ __global__ void __launch_bounds__(256) bn_bwd_chan_kernel(const BnBwdParams<T> p
   for (int op = threadIdx.x; op < outP; op += blockDim.x) {
     float yv[NP][8], dz[NP][8];
     long long ip[NP];
-    bn_dz<POOL, T>(p, op, g, sc, sh, yv, dz, ip);
+    if constexpr (ODD) bn_dz_odd<T>(p, op, g, sc, sh, yv, dz, ip);
+    else bn_dz<POOL, T>(p, op, g, sc, sh, yv, dz, ip);
 #pragma unroll
     for (int q = 0; q < NP; ++q) {
+      if constexpr (ODD) { if (ip[q] < 0) continue; }
       float r[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -1548,6 +1611,8 @@ int slb_preload_elementwise() {
   { auto k = bn_bwd_apply_kernel<true, T>; SLB_PRELOAD(k); } { auto k = bn_bwd_apply_kernel<false, T>; SLB_PRELOAD(k); } \
   { auto k = bn_bwd_fused_kernel<true, T>; SLB_PRELOAD(k); } { auto k = bn_bwd_fused_kernel<false, T>; SLB_PRELOAD(k); } \
   { auto k = bn_bwd_chan_kernel<true, T>; SLB_PRELOAD(k); } { auto k = bn_bwd_chan_kernel<false, T>; SLB_PRELOAD(k); } \
+  { auto k = bn_relu_pool_fwd_kernel<T, false, true>; SLB_PRELOAD(k); } { auto k = bn_bwd_chan_kernel<true, T, true>; SLB_PRELOAD(k); } \
+  { auto k = bn_bwd_reduce_kernel<true, T, true>; SLB_PRELOAD(k); } { auto k = bn_bwd_apply_kernel<true, T, true>; SLB_PRELOAD(k); } \
   { auto k = col_stats_kernel<T>; SLB_PRELOAD(k); } { auto k = conv_finalize_kernel<T>; SLB_PRELOAD(k); } \
   { auto k = conv3x3_small_fwd_kernel<3, 64, T>; SLB_PRELOAD(k); } { auto k = conv3x3_small_fwd_kernel<1, 64, T>; SLB_PRELOAD(k); } \
   { auto k = conv3x3_small_fwd_kernel<3, 32, T>; SLB_PRELOAD(k); } { auto k = conv3x3_small_fwd_kernel<1, 32, T>; SLB_PRELOAD(k); } \
@@ -1613,6 +1678,11 @@ static int bn_fwd_t(const void* y, const float* sum, const float* sumsq, const f
   BnFwdParams<T> p = {reinterpret_cast<const T*>(y), sum, sumsq, gamma, beta, running_mean, running_var, nbt,
                       save_mean, save_invstd, reinterpret_cast<T*>(out), P, C, H, W, relu, pool, momentum, eps,
                       update_running, identity, ticket, flag, seq, hint};
+  if (pool && ((H | W) & 1)) {                    // odd map: floor(H/2) x floor(W/2) windows
+    const long long work = (long long)(P / (H * W)) * (H >> 1) * (W >> 1) * (C / 8);
+    launch_k(bn_relu_pool_fwd_kernel<T, false, true>, grid_for(work, 256, 132 * 4), 256, 2 * C * sizeof(float), st, p);
+    return last_err();
+  }
   const long long work = (pool ? (long long)P / 4 : P) * (C / 8);
   launch_k(bn_relu_pool_fwd_kernel<T>, grid_for(work, 256, 132 * 4), 256, 2 * C * sizeof(float), st, p);
   return last_err();
@@ -1624,6 +1694,7 @@ int slb_bn_relu_pool_fwd(const void* y, const float* sum, const float* sumsq, co
                          int update_running, int identity, uint32_t* ticket, uint32_t* flag, uint32_t* seq, uint32_t* hint,
                          int dtype, cudaStream_t st) {
   if (C % 8) return -1;
+  if (pool && ((H | W) & 1) && (H < 1 || W < 1 || P % (H * W))) return -1;
   if (dtype == 1)
     return bn_fwd_t<float>(y, sum, sumsq, gamma, beta, running_mean, running_var, nbt, save_mean, save_invstd, out, P, C, H, W,
                            relu, pool, momentum, eps, update_running, identity, ticket, flag, seq, hint, st);
@@ -1648,6 +1719,7 @@ int slb_bn_relu_pool_infer(const void* y, const float* gamma, const float* beta,
                            const float* running_var, void* out, int P, int C, int H, int W, int relu, int pool, float eps,
                            int dtype, cudaStream_t st) {
   if (C % 8 || gamma == nullptr || beta == nullptr || running_mean == nullptr || running_var == nullptr) return -1;
+  if (pool && ((H | W) & 1)) return -2;          // the eval plan pools even maps only
   if (dtype == 1) return bn_infer_t<float>(y, gamma, beta, running_mean, running_var, out, P, C, H, W, relu, pool, eps, st);
   return bn_infer_t<__nv_bfloat16>(y, gamma, beta, running_mean, running_var, out, P, C, H, W, relu, pool, eps, st);
 }
@@ -1674,9 +1746,22 @@ static int bn_bwd_t(const void* dout, const void* y, const float* gamma, const f
   const int tx = C / 8;
   const int ty = tx >= 256 ? 1 : 256 / tx;
   dim3 block(tx, ty);
-  const long long outP = pool ? (long long)P / 4 : P;
+  const bool odd = pool && ((H | W) & 1);
+  // odd map: positions on the ceil(H/2) x ceil(W/2) grid, so the dropped last row / column also receives its dy
+  const long long outP = odd ? (long long)(P / (H * W)) * ((H + 1) >> 1) * ((W + 1) >> 1) : (pool ? (long long)P / 4 : P);
   const int grid = grid_for(outP, ty, 132 * 2);
   if (p.det.part == nullptr || (long long)grid * 2 * C > p.det.cap) return -30;
+  if (odd) {                                        // channel-owned or two-pass kernels; the grid-barrier kernel is even-only
+    if (grid_bar != nullptr && !identity) return -2;
+    if (!identity && !skip_reduce && P <= bn_bwd_chan_max_p()) {
+      const int thr = outP >= 256 ? 256 : (outP >= 128 ? 128 : 64);
+      launch_k(bn_bwd_chan_kernel<true, T, true>, C / 8, thr, 0, st, p);
+      return last_err();
+    }
+    if (!identity && !skip_reduce) launch_k(bn_bwd_reduce_kernel<true, T, true>, grid, block, 2 * C * sizeof(float), st, p);
+    launch_k(bn_bwd_apply_kernel<true, T, true>, grid, block, 0, st, p);
+    return last_err();
+  }
   if (grid_bar != nullptr && !identity) {          // one launch: reduce -> grid barrier -> apply
     // the software barrier needs every block co-resident: cap the grid at (SMs - 4) x measured occupancy
     static int cap[2] = {0, 0};
@@ -1715,6 +1800,7 @@ int slb_bn_relu_pool_bwd(const void* dout, const void* y, const float* gamma, co
                          const float* save_invstd, float* dgamma, float* dbeta, void* dy, int P, int C, int H, int W, int relu,
                          int pool, int identity, uint32_t* grid_bar, int dtype, cudaStream_t st) {
   if (C % 8 || C > 2048) return -1;
+  if (pool && ((H | W) & 1) && (H < 1 || W < 1 || P % (H * W))) return -1;
   if (dtype == 1)
     return bn_bwd_t<float>(dout, y, gamma, beta, save_mean, save_invstd, dgamma, dbeta, dy, P, C, H, W, relu, pool, identity, grid_bar, st);
   return bn_bwd_t<__nv_bfloat16>(dout, y, gamma, beta, save_mean, save_invstd, dgamma, dbeta, dy, P, C, H, W, relu, pool, identity, grid_bar, st);

@@ -229,9 +229,26 @@ __device__ __forceinline__ void stat_terms(const GemmParams& p, int row, bool ro
   }  // BNB
 }
 
+// Ragged pixel tiles (RAG): a tile is one padded power-of-two box (tb x th x tw pixel slots, tw >= W, th >= min(H, ...))
+// at (b0, h0, 0) of the NHWC tensor; slots outside the tensor are TMA out-of-bounds zero fill.  Tile t of a conv has
+// b0 = (t / tiles_h) * tb and h0 = (t % tiles_h) * th, tiles_h = ceil(H / th); a wgrad K step is one such box.
+__device__ __forceinline__ int rag_tiles_h(const GemmParams& p) { return (p.H + p.th - 1) / p.th; }
+
+// Row r of ragged conv tile `t` is pixel (b0 + r / (tw th), h0 + (r / tw) % th, r % tw); false for padding slots.
+__device__ __forceinline__ bool rag_row(const GemmParams& p, int t, int r, long long& off) {
+  const int tiles_h = rag_tiles_h(p);
+  const int b = (t / tiles_h) * p.tb + r / (p.tw * p.th);
+  const int h = (t % tiles_h) * p.th + (r / p.tw) % p.th;
+  const int w = r % p.tw;
+  off = ((static_cast<long long>(b) * p.H + h) * p.W + w) * p.ldo;
+  return b < p.M / (p.H * p.W) && h < p.H && w < p.W;
+}
+
 // BNB: instantiate the upstream-BatchNorm-backward epilogue (dgrad only).  A separate instantiation on purpose: with the
 // code in the common kernel every conv paid ~1.8 % (205 vs 154 registers; same-box A/B, profiles/README.md).
-template <int MODE, int BLOCK_N, typename T, bool BNB = false>
+// RAG: ragged pixel tiles (above) for maps whose width does not divide the tile; also a separate instantiation, so the
+// power-of-two kernels keep their code.  The host gives a ragged conv k_split == 1 and no statistics, BNB or publish.
+template <int MODE, int BLOCK_N, typename T, bool BNB = false, bool RAG = false>
 __global__ void __launch_bounds__(288, 1)
 umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
@@ -295,11 +312,18 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const int tap = it / kc_per_tap, kc = it - tap * kc_per_tap;
             int dh = tap / 3 - 1, dw = tap % 3 - 1;
             if (p.flip) { dh = -dh; dw = -dw; }
-            // pixel tile origin: 128 consecutive NHWC pixels starting at m0
-            const int pix_per_img = p.H * p.W;
-            const int b0 = m0 / pix_per_img;
-            const int rem = m0 - b0 * pix_per_img;
-            const int h0 = rem / p.W;
+            int b0, h0;
+            if constexpr (RAG) {
+              const int tiles_h = rag_tiles_h(p);
+              b0 = (m_tile / tiles_h) * p.tb;
+              h0 = (m_tile % tiles_h) * p.th;
+            } else {
+              // pixel tile origin: 128 consecutive NHWC pixels starting at m0
+              const int pix_per_img = p.H * p.W;
+              b0 = m0 / pix_per_img;
+              const int rem = m0 - b0 * pix_per_img;
+              h0 = rem / p.W;
+            }
             tma_load_4d(sa, &tmA, &full_bar[stage], kc * KE, dw, h0 + dh, b0);
             if (!p.b_mn) {
               tma_load_2d(sb, &tmB, &full_bar[stage], tap * p.b_row_stride + kc * KE, n0);
@@ -309,12 +333,20 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 tma_load_2d(sb + g * GROUP_BYTES, &tmB, &full_bar[stage], tap * p.b_row_stride + n0 + g * KE, kc * KE);
             }
           } else if constexpr (MODE == MODE_WGRAD) {
-            // K iteration = KE consecutive pixels starting at it*KE
-            const int pix0 = it * KE;
-            const int pix_per_img = p.H * p.W;
-            const int b0 = pix0 / pix_per_img;
-            const int rem = pix0 - b0 * pix_per_img;
-            const int h0 = rem / p.W;
+            int b0, h0;
+            if constexpr (RAG) {
+              // K iteration = one padded box of KE pixel slots; empty slots are zero in both operands
+              const int tiles_h = rag_tiles_h(p);
+              b0 = (it / tiles_h) * p.tb;
+              h0 = (it % tiles_h) * p.th;
+            } else {
+              // K iteration = KE consecutive pixels starting at it*KE
+              const int pix0 = it * KE;
+              const int pix_per_img = p.H * p.W;
+              b0 = pix0 / pix_per_img;
+              const int rem = pix0 - b0 * pix_per_img;
+              h0 = rem / p.W;
+            }
 #pragma unroll
             for (int g = 0; g < 128 / KE; ++g) {
               const int r = m0 + g * KE;
@@ -376,7 +408,9 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       // warp-private transpose tile for the statistics, in front of the accumulator tile
       float* s_tr = reinterpret_cast<float*>(smem) + warp * (32 * 33);
       static_assert(L::ACC_OFF >= 4 * 32 * 33 * 4, "transpose tiles must fit in front of the accumulator tile");
-      const bool row_ok = row < p.M;
+      constexpr bool RAG_ROWS = RAG && MODE == MODE_CONV;        // a ragged wgrad keeps its [Cout][3][3][Cin] rows
+      long long rag_off = 0;
+      const bool row_ok = RAG_ROWS ? rag_row(p, m_tile, q * 32 + lane_id(), rag_off) : row < p.M;
       long long row_off;
       bool row_store = row_ok;
       if (p.rmod > 0) {
@@ -384,7 +418,7 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         row_off = lo * p.rmul1 + hi * p.rmul2;
         row_store = row_ok && hi < p.m_valid_mod;
       } else {
-        row_off = static_cast<long long>(row) * p.ldo;
+        row_off = RAG_ROWS ? rag_off : static_cast<long long>(row) * p.ldo;
       }
       // split-K with in-kernel finalisation (tile_counters): every K slice stores its partial tile into slice z of `out`
       // ([k_split][M][ldo]); the last slice of the tile to arrive adds the k_split partials in slice order.  Without
@@ -686,9 +720,9 @@ static int tmap_nhwc(CUtensorMap* m, const void* base, int B, int H, int W, int 
   return make_tmap(m, base, 4, dims, str, box, dtype, mn_major);
 }
 
-template <int MODE, int BN, typename T, bool BNB = false>
+template <int MODE, int BN, typename T, bool BNB = false, bool RAG = false>
 static int launch(const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p_in, dim3 grid, cudaStream_t st) {
-  auto k = umma_gemm_kernel<MODE, BN, T, BNB>;
+  auto k = umma_gemm_kernel<MODE, BN, T, BNB, RAG>;
   GemmParams p = p_in;
   p.det = slb_det(st);
   if (p.det.part == nullptr) return -30;
@@ -706,10 +740,21 @@ static int launch(const CUtensorMap& a, const CUtensorMap& b, const GemmParams& 
   return e == cudaSuccess ? 0 : -static_cast<int>(e) - 2000;
 }
 
-template <int MODE>
+template <int MODE, bool RAG = false>
 static int dispatch_bn(int bn, int dtype, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, dim3 grid,
                        cudaStream_t st) {
   using bf = __nv_bfloat16;
+  if constexpr (RAG) {                            // ragged pixel tiles: bf16 conv / dgrad / wgrad
+    static_assert(MODE != MODE_GEMM, "ragged tiles are a conv geometry");
+    if (dtype != 0 || p.bnb_y != nullptr) return -13;
+    switch (bn) {
+      case 32: if constexpr (MODE == MODE_CONV) return launch<MODE, 32, bf, false, true>(a, b, p, grid, st); else return -3;
+      case 64: return launch<MODE, 64, bf, false, true>(a, b, p, grid, st);
+      case 128: return launch<MODE, 128, bf, false, true>(a, b, p, grid, st);
+      case 256: return launch<MODE, 256, bf, false, true>(a, b, p, grid, st);
+      default: return -3;
+    }
+  }
   if (dtype == 1) {                               // fp32 tensors, wgmma tf32 (conv fwd / dgrad / wgrad only)
     if constexpr (MODE == MODE_GEMM) return -5;
     else {
@@ -742,10 +787,10 @@ static int dispatch_bn(int bn, int dtype, const CUtensorMap& a, const CUtensorMa
   }
 }
 
-template <int MODE, int BN, typename T, bool BNB = false>
+template <int MODE, int BN, typename T, bool BNB = false, bool RAG = false>
 static int preload_one() {
   cudaFuncAttributes a;
-  return cudaFuncGetAttributes(&a, umma_gemm_kernel<MODE, BN, T, BNB>) == cudaSuccess ? 0 : 1;
+  return cudaFuncGetAttributes(&a, umma_gemm_kernel<MODE, BN, T, BNB, RAG>) == cudaSuccess ? 0 : 1;
 }
 
 static void pixel_box(int H, int W, int pixels, int* tb, int* th, int* tw) {
@@ -753,6 +798,24 @@ static void pixel_box(int H, int W, int pixels, int* tb, int* th, int* tw) {
   int rows = pixels / W;           // full-width rows in the tile
   if (rows <= H) { *th = rows; *tb = 1; }
   else { *th = H; *tb = rows / H; }
+}
+
+// Does pixel_box tile the map exactly, so that tile t is the `pixels` consecutive NHWC pixels from t * pixels?  Power-of-
+// two maps do.  Every other map (W = 28, 14, 7, 3, ...) takes the ragged instantiation with padded_box.
+static bool pixel_box_exact(int H, int W, int pixels) {
+  if (W > pixels || pixels % W != 0) return false;
+  const int rows = pixels / W;
+  return rows <= H ? H % rows == 0 : rows % H == 0;
+}
+
+// Padded power-of-two box of `pixels` slots for W <= pixels: tw = the smallest power of two >= W, th = min(the smallest
+// power of two >= H, pixels / tw), tb = the rest.  Equal to pixel_box for power-of-two H and W.
+static void padded_box(int H, int W, int pixels, int* tb, int* th, int* tw) {
+  int w = 1, h = 1;
+  while (w < W) w <<= 1;
+  while (h < H) h <<= 1;
+  if (h > pixels / w) h = pixels / w;
+  *tw = w; *th = h; *tb = pixels / (w * h);
 }
 
 }  // namespace slb
@@ -772,7 +835,19 @@ int slb_preload_gemm() {
   bad += preload_one<MODE_CONV, 64, bf, true>() + preload_one<MODE_CONV, 128, bf, true>() + preload_one<MODE_CONV, 256, bf, true>();
   bad += preload_one<MODE_CONV, 64, float>() + preload_one<MODE_CONV, 128, float>() + preload_one<MODE_CONV, 256, float>() + preload_one<MODE_CONV, 32, float>();
   bad += preload_one<MODE_WGRAD, 64, float>() + preload_one<MODE_WGRAD, 128, float>() + preload_one<MODE_WGRAD, 256, float>() + preload_one<MODE_WGRAD, 32, float>();
+  bad += preload_one<MODE_CONV, 32, bf, false, true>() + preload_one<MODE_CONV, 64, bf, false, true>() + preload_one<MODE_CONV, 128, bf, false, true>() + preload_one<MODE_CONV, 256, bf, false, true>();
+  bad += preload_one<MODE_WGRAD, 64, bf, false, true>() + preload_one<MODE_WGRAD, 128, bf, false, true>() + preload_one<MODE_WGRAD, 256, bf, false, true>();
   return bad;
+}
+
+// The pixel box of a conv tile (pixels = 128) or wgrad K step (pixels = 64 bf16 / 32 fp32): out = {tb, th, tw, ragged}.
+// ragged = 0: pixel_box over consecutive pixels; 1: padded_box; -1: no box (W > pixels).
+void slb_conv_pixel_box(int H, int W, int pixels, int padded, int* out) {
+  int tb = 0, th = 0, tw = 0, rag = 0;
+  if (W < 1 || H < 1 || W > pixels) rag = -1;
+  else if (!padded && pixel_box_exact(H, W, pixels)) pixel_box(H, W, pixels, &tb, &th, &tw);
+  else { padded_box(H, W, pixels, &tb, &th, &tw); rag = 1; }
+  out[0] = tb; out[1] = th; out[2] = tw; out[3] = rag;
 }
 
 // y[B,H,W,Cout] (pre-BN) = conv3x3(x[B,H,W,Cin], w[Cout][3][3][Cin]) + bias ; optional per-channel
@@ -830,9 +905,17 @@ static int conv_igemm_impl(const void* x, const void* w, void* y, const float* b
   const int KE = 128 / esize(dtype);
   if (Ca % KE != 0 || Nout % 32 != 0) return -10;
   const int M = B * H * W;
-  if (128 % W != 0 && W % 128 != 0) return -11;
+  if (B < 1 || H < 1 || W < 1 || W > 128) return -11;
+  const bool rag = !pixel_box_exact(H, W, 128);
+  if (rag) {
+    // ragged tiles: single K slice, plain epilogue (split-K, BN statistics, fused BN-backward sums and the publish
+    // are power-of-two-only options), bf16 only
+    if (dtype != 0) return -13;
+    if (k_split > 1 || col_sum != nullptr || col_sumsq != nullptr || bnb != nullptr || pub != nullptr) return -14;
+  }
   int tb, th, tw;
-  pixel_box(H, W, 128, &tb, &th, &tw);
+  if (rag) padded_box(H, W, 128, &tb, &th, &tw);
+  else pixel_box(H, W, 128, &tb, &th, &tw);
   if (tw * th * tb != 128) return -12;
   int bn = block_n > 0 ? block_n : (Nout >= 256 ? 256 : Nout);   // 32, 64, 128, 256
   if (bn > Nout) bn = Nout;
@@ -874,6 +957,10 @@ static int conv_igemm_impl(const void* x, const void* w, void* y, const float* b
   }
   p.trace = g_gemm_trace;
   if (pub != nullptr) { p.pub_ticket = pub->ticket; p.pub_flag = pub->flag; p.pub_seq = pub->seq; }
+  if (rag) {
+    dim3 grid(((B + tb - 1) / tb) * ((H + th - 1) / th), Nout / bn, 1);
+    return dispatch_bn<MODE_CONV, true>(bn, dtype, ta, tbm, p, grid, st);
+  }
   dim3 grid((M + 127) / 128, Nout / bn, k_split);
   return dispatch_bn<MODE_CONV>(bn, dtype, ta, tbm, p, grid, st);
 }
@@ -889,9 +976,12 @@ int slb_conv3x3_wgrad(const void* x, const void* dy, float* dw, int B, int H, in
   const int KE = 128 / esize(dtype);
   if (Cin % KE != 0 || Cout % KE != 0) return -10;
   const int pixels = B * H * W;
-  if (KE % W != 0) return -11;
+  if (B < 1 || H < 1 || W < 1 || W > KE) return -11;
+  const bool rag = !pixel_box_exact(H, W, KE);     // ragged: one K step = one padded box (bf16 only)
+  if (rag && dtype != 0) return -13;
   int tb, th, tw;
-  pixel_box(H, W, KE, &tb, &th, &tw);
+  if (rag) padded_box(H, W, KE, &tb, &th, &tw);
+  else pixel_box(H, W, KE, &tb, &th, &tw);
   if (tw * th * tb != KE) return -12;
   int bn = block_n > 0 ? block_n : (Cin >= 128 ? 128 : Cin);
   if (bn > Cin) bn = Cin;
@@ -904,6 +994,7 @@ int slb_conv3x3_wgrad(const void* x, const void* dy, float* dw, int B, int H, in
   GemmParams p = {};
   const int rows = 9 * Cout;
   p.M = ((rows + 127) / 128) * 128; p.N = Cin; p.k_iters = (pixels + KE - 1) / KE;   // tail pixels are TMA zero-fill
+  if (rag) p.k_iters = ((B + tb - 1) / tb) * ((H + th - 1) / th);
   const int m_tiles = p.M / 128, n_tiles = Cin / bn;
   if (k_split <= 0) {
     int sms = 0, dev = 0;
@@ -926,6 +1017,7 @@ int slb_conv3x3_wgrad(const void* x, const void* dy, float* dw, int B, int H, in
   p.C = Cout; p.tw = tw; p.th = th; p.tb = tb; p.H = H; p.W = W; p.Cout = Cout;
   p.trace = g_gemm_trace;
   dim3 grid(m_tiles, n_tiles, k_split);
+  if (rag) return dispatch_bn<MODE_WGRAD, true>(bn, dtype, ta, tbm, p, grid, st);
   return dispatch_bn<MODE_WGRAD>(bn, dtype, ta, tbm, p, grid, st);
 }
 

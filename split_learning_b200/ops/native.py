@@ -206,6 +206,15 @@ def conv_finalize(acc, bias, y, col_sum, col_sumsq):
                                    _stream()), "conv_finalize")
 
 
+def conv_pixel_box(H: int, W: int, pixels: int = 128, padded: bool = False):
+    """(tb, th, tw, ragged) of a conv tile (``pixels`` = 128) or wgrad K step (64 bf16 / 32 fp32 pixels): the box the
+    kernels load for an H x W map.  ragged 0 = consecutive pixels (power-of-two maps), 1 = padded power-of-two box
+    (``padded=True`` forces it), -1 = no box (W > pixels)."""
+    out = (c_int * 4)()
+    lib().slb_conv_pixel_box(c_int(H), c_int(W), c_int(pixels), c_int(int(padded)), out)
+    return tuple(out)
+
+
 def conv3x3_wgrad(x, dy, dw_f32, k_split: int = 0, block_n: int = 0):
     """dw [Cout,3,3,Cin] fp32 (+)= x^T (*) dy.  Split-K slices accumulate with red.add (caller zeroes dw); a layer
     whose K fits one slice is written with plain stores."""

@@ -1,6 +1,9 @@
 """Native execution of the conv / BN / ReLU tables that the compiled VGG plan (``b200_executor``) does not cover —
 MobileNetv1_CIFAR10 / MobileNetv1_MNIST of the Vanilla_SL variant (other/Vanilla_SL/src/model/MobileNetv1_CIFAR10.py:5-185:
-dense 3x3 convs with stride 1 or 2, 1x1 convs, 32-channel layers, one max-pool, one Linear).
+dense 3x3 convs with stride 1 or 2, 1x1 convs, 32-channel layers, one max-pool, one Linear) and VGG16_MNIST
+(other/Vanilla_SL/src/model/VGG16_MNIST.py: 28 -> 14 -> 7 -> 3 -> 1 pixel maps, four 2x2 max-pools of which the last two
+pool odd maps, dropout, three Linears).  The compiled plan keeps its power-of-two-width rule, so VGG16_MNIST trains here
+and has no native eval plan.
 
 Same scheme as ``token_native``: the module tree (parameter names, state-dict, checkpoints) is untouched, the stage's
 ``forward`` is re-bound to a small NHWC/bf16 program whose heavy ops are ``torch.autograd.Function``s over the
@@ -8,13 +11,17 @@ hand-written sm_90a kernels:
 
 * 3x3 conv  -> the wgmma implicit-GEMM kernel (forward, dgrad with mirrored taps, split-K wgrad).  Channel counts
   that are not multiples of 64 are zero-padded in the bf16 weight view; stride 2 is computed at stride 1 and
-  sub-sampled (4 of the 27 convs), its backward scatters into a zero tensor;
+  sub-sampled (4 of the 27 convs), its backward scatters into a zero tensor.  Maps whose width does not divide the
+  128-pixel tile (28, 14, 7, 3) run the ragged instantiation: padded power-of-two pixel boxes, TMA zero fill;
 * 1x1 conv  -> the wgmma GEMM of ``ops.nn.linear`` on the NHWC view (no im2col, no layout change);
 * first conv (Cin = 1 or 3, NCHW fp32 input) -> ``conv3x3_small_fwd_kernel`` / ``conv3x3_small_wgrad_kernel``;
 * BatchNorm(train) + ReLU (+ MaxPool2) -> ``col_stats`` + ``bn_relu_pool_fwd`` / ``bn_relu_pool_bwd`` (running
-  statistics and ``num_batches_tracked`` updated by the kernel);
-* Linear -> ``ops.nn.linear``.
-Stage boundaries stay NCHW fp32 (the reference's wire format).  ``TorchExecutor(native=True)`` captures whole steps of
+  statistics and ``num_batches_tracked`` updated by the kernel; odd maps pool with floor semantics, 7 -> 3 and 3 -> 1,
+  and the dropped last row / column still receives its BatchNorm gradient);
+* Linear (+ ReLU) -> ``ops.nn.linear`` (ReLU in the GEMM epilogue); Dropout -> ``ops.nn.dropout`` (hash dropout, seeded
+  per replay under CUDA graphs).
+Activations are bf16 (VGG16_MNIST included: there is no tf32 flavour of this program).  Stage boundaries stay NCHW fp32
+(the reference's wire format).  ``TorchExecutor(native=True)`` captures whole steps of
 this program into CUDA graphs exactly as for the token models.
 """
 from __future__ import annotations
@@ -26,6 +33,7 @@ import torch
 import torch.nn as nn
 
 from ..models import mobilenet as M
+from ..models import vgg16 as V
 from ..ops import native as N
 from ..ops import nn as F
 
@@ -33,7 +41,7 @@ _BF = torch.bfloat16
 
 
 def supports(model: nn.Module) -> bool:
-    return isinstance(model, (M.MobileNetv1_CIFAR10, M.MobileNetv1_MNIST))
+    return isinstance(model, (M.MobileNetv1_CIFAR10, M.MobileNetv1_MNIST, V.VGG16_MNIST))
 
 
 def _c64(c: int) -> int:
@@ -173,14 +181,14 @@ class _BnActFn(torch.autograd.Function):
 # ------------------------------------------------------------------------------------------------ stage program
 def _program(model) -> List[Tuple]:
     """Group the owned layer indices into fused ops: ('stem'|'conv3'|'conv1', i) ('bn', i, relu, pool)
-    ('relu',) ('pool',) ('flatten',) ('linear', i)."""
+    ('relu',) ('pool',) ('flatten',) ('dropout', i) ('linear', i) ('linear', i, 'relu') (a Linear followed by a ReLU)."""
     idx = list(model.owned_indices())
     kinds = {i: model.LAYERS[i - 1].kind for i in idx}
     ops, k = [], 0
     while k < len(idx):
         i = idx[k]
         kind = kinds[i]
-        if kind == "conv":
+        if kind in ("conv", "conv3x3"):
             mod = getattr(model, f"layer{i}")
             if mod.kernel_size == (1, 1):
                 ops.append(("conv1", i))
@@ -197,9 +205,13 @@ def _program(model) -> List[Tuple]:
         elif kind in ("relu", "maxpool2", "flatten"):
             ops.append(({"relu": "relu", "maxpool2": "pool", "flatten": "flatten"}[kind],))
             k += 1
-        elif kind == "linear":
-            ops.append(("linear", i))
+        elif kind == "dropout":
+            ops.append(("dropout", i))
             k += 1
+        elif kind == "linear":
+            relu = k + 1 < len(idx) and kinds[idx[k + 1]] == "relu"
+            ops.append(("linear", i, "relu") if relu else ("linear", i))
+            k += 1 + int(relu)
         else:
             raise N.NativeError(f"no native op for layer kind {kind!r}")
     return ops
@@ -245,9 +257,11 @@ def _forward(self, x, **_):
                 x = x.permute(0, 3, 1, 2)
                 nhwc = False
             x = x.reshape(x.shape[0], -1)
+        elif name == "dropout":
+            x = F.dropout(x, getattr(self, f"layer{op[1]}").p, self.training)
         elif name == "linear":
             mod = getattr(self, f"layer{op[1]}")
-            x = F.linear(x, mod.weight, mod.bias)
+            x = F.linear(x, mod.weight, mod.bias, act=op[2] if len(op) > 2 else None)
     if nhwc:
         x = x.permute(0, 3, 1, 2)
     return x
