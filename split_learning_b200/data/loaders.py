@@ -228,9 +228,16 @@ def resident_test_loader(data_name: str, device, synthetic: Optional[bool] = Non
     """The test split of ``data_loader(data_name, train=False)`` held in HBM: the same samples in the same order and batches
     (100, short batch last), so results compare sample for sample.  Real CIFAR10: the uint8 [10000, 32, 32, 3] split is
     uploaded once and each batch is one ``image_batch`` launch with crop and flip off (= ToTensor + Normalize).  Synthetic:
-    the same ``SyntheticDataset`` test samples, resident as fp32."""
+    the same ``SyntheticDataset`` test samples, resident as fp32.  AGNEWS / EMOTION: the int64 ``input_ids`` of one pass over
+    the host test loader (synthetic or the tokenised CSV), stacked and uploaded once; batches of 20, short batch last."""
     from .gpu_loader import CIFAR_MEAN, CIFAR_STD, GpuImageLoader, ResidentBatches
     name = str(data_name).upper()
+    if name in ("AGNEWS", "EMOTION"):
+        ids, labels = [], []
+        for batch in data_loader(name, train=False, synthetic=synthetic, root=root, seed=seed):
+            ids.append(batch["input_ids"].long())
+            labels.append(torch.as_tensor(batch["labels"]).long())
+        return ResidentBatches(torch.cat(ids), torch.cat(labels), DATASET_SHAPES[name][3], device)
     if name != "CIFAR10":
         raise ValueError(f"no resident test split for {data_name}")
     if synthetic is None:

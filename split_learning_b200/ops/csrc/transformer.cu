@@ -13,6 +13,8 @@
 //   act_bwd_kernel, colsum_kernel      GELU / tanh / ReLU backward, bias gradient
 //   dropout_bf16_kernel                hash dropout (same kernel re-applies the mask in backward)
 //   embed3_fwd_kernel / embed3_bwd_kernel   word + position + token-type embedding gather / scatter-add
+//   patch_rows_kernel, vit_tokens_kernel, ln_rows_fwd_kernel   the eval program's ViT patch rows, CLS + position
+//       assembly and the head LayerNorm of the CLS rows (train/token_eval.py)
 #include "sm90.cuh"
 
 namespace slb {
@@ -553,7 +555,83 @@ embed3_bwd_kernel(const long long* __restrict__ ids, const long long* __restrict
   }
 }
 
+// ----------------------------------------------------------------------------- eval-mode token assembly (ViT / BERT)
+// ViT patch embedding as a GEMM operand: x fp32 NCHW [B][C][H][W] -> rows [B * (H/p) * (W/p)][C * p * p] bf16, row
+// (b, gy, gx), column (c, py, px) — the unfold order of a Conv2d(kernel = stride = p) weight [E][C][p][p].
+__global__ void __launch_bounds__(256)
+patch_rows_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, long long n, int C, int H, int W, int p) {
+  pdl_wait();
+  const int K = C * p * p, gw = W / p, gh = H / p;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long row = i / K;
+    const int k = static_cast<int>(i - row * K);
+    const int gx = static_cast<int>(row % gw);
+    const long long t = row / gw;
+    const int gy = static_cast<int>(t % gh);
+    const long long b = t / gh;
+    const int c = k / (p * p), r = k - c * p * p, py = r / p, px = r - py * p;
+    out[i] = __float2bfloat16_rn(x[((b * C + c) * H + gy * p + py) * static_cast<long long>(W) + gx * p + px]);
+  }
+}
+
+// ViT token sequence: out[b][0] = cls + pos[0], out[b][1 + i] = pe[b * P + i] + pos[1 + i]  (fp32 adds, one bf16
+// rounding: the values torch.cat([cls, pe]) + pos_embed holds before the first block casts it).  One warp per token.
+__global__ void __launch_bounds__(256)
+vit_tokens_kernel(const __nv_bfloat16* __restrict__ pe, const float* __restrict__ cls, const float* __restrict__ pos,
+                  __nv_bfloat16* __restrict__ out, int B, int P, int E) {
+  pdl_wait();
+  const int t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (t >= B * (P + 1)) return;
+  const int b = t / (P + 1), s = t - b * (P + 1);
+  const float2* q = reinterpret_cast<const float2*>(pos + static_cast<long long>(s) * E);
+  __nv_bfloat162* o = reinterpret_cast<__nv_bfloat162*>(out + static_cast<long long>(t) * E);
+  if (s == 0) {
+    const float2* c2 = reinterpret_cast<const float2*>(cls);
+    for (int i = lane_id(); i < (E >> 1); i += 32) {
+      const float2 a = c2[i], d = q[i];
+      o[i] = __floats2bfloat162_rn(a.x + d.x, a.y + d.y);
+    }
+  } else {
+    const __nv_bfloat162* e2 = reinterpret_cast<const __nv_bfloat162*>(pe + (static_cast<long long>(b) * P + s - 1) * E);
+    for (int i = lane_id(); i < (E >> 1); i += 32) {
+      const float2 a = __bfloat1622float2(e2[i]), d = q[i];
+      o[i] = __floats2bfloat162_rn(a.x + d.x, a.y + d.y);
+    }
+  }
+}
+
+// LayerNorm of rows with a pitch: y[r] = LN(x[r * ldx]) * gamma + beta, one warp per row.  The CLS row of every sequence
+// (ldx = S * D) is normalised straight out of the encoder output, without a gather.  Same arithmetic as ln_fwd_kernel
+// without its prologue, so a row gives the same bits through either kernel; no mean / rstd is kept (inference only).
+__global__ void __launch_bounds__(256)
+ln_rows_fwd_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const float* __restrict__ gamma,
+                   const float* __restrict__ beta, __nv_bfloat16* __restrict__ y, int rows, int D, float eps) {
+  pdl_wait();
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const int lane = lane_id(), D2 = D >> 1;
+  const __nv_bfloat162* x2 = reinterpret_cast<const __nv_bfloat162*>(x + static_cast<long long>(row) * ldx);
+  __nv_bfloat162* y2 = reinterpret_cast<__nv_bfloat162*>(y + static_cast<long long>(row) * D);
+  float s1 = 0.f, s2 = 0.f;
+  for (int i = lane; i < D2; i += 32) {
+    const float2 w = __bfloat1622float2(x2[i]);
+    s1 += w.x + w.y;
+    s2 += w.x * w.x + w.y * w.y;
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) { s1 += __shfl_xor_sync(0xffffffffu, s1, o); s2 += __shfl_xor_sync(0xffffffffu, s2, o); }
+  const float mu = s1 / D, var = fmaxf(s2 / D - mu * mu, 0.f), rs = rsqrtf(var + eps);
+  for (int i = lane; i < D2; i += 32) {
+    const float2 v = __bfloat1622float2(x2[i]);
+    const float2 g = reinterpret_cast<const float2*>(gamma)[i], bb = reinterpret_cast<const float2*>(beta)[i];
+    y2[i] = __floats2bfloat162_rn((v.x - mu) * rs * g.x + bb.x, (v.y - mu) * rs * g.y + bb.y);
+  }
+}
+
 // ----------------------------------------------------------------------------- host side
+static bool misaligned(const void* ptr, uintptr_t bytes) { return ptr == nullptr || (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)); }
+
 typedef CUresult (*PFN_encodeTiled3)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                      const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                      CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -726,6 +804,35 @@ int slb_embed3_bwd(const long long* ids, const long long* tts, const void* g, fl
   return check_launch();
 }
 
+// x fp32 [B][C][H][W] -> out bf16 [B * (H/p) * (W/p)][C * p * p]; C * p * p % 8 == 0 (the row pitch of a GEMM operand)
+int slb_patch_rows(const float* x, void* out, int B, int C, int H, int W, int p, cudaStream_t st) {
+  if (B < 1 || C < 1 || p < 1 || H < p || W < p || H % p || W % p) return -3;
+  if ((C * p * p) % 8 || misaligned(x, 4) || misaligned(out, 16)) return -4;
+  const long long n = static_cast<long long>(B) * C * H * W;
+  long long grid = (n + 255) / 256;
+  if (grid > 132 * 16) grid = 132 * 16;
+  patch_rows_kernel<<<static_cast<int>(grid), 256, 0, st>>>(x, reinterpret_cast<__nv_bfloat16*>(out), n, C, H, W, p);
+  return check_launch();
+}
+// pe bf16 [B*P][E], cls fp32 [E], pos fp32 [P+1][E] -> out bf16 [B*(P+1)][E]; E even
+int slb_vit_tokens(const void* pe, const float* cls, const float* pos, void* out, int B, int P, int E, cudaStream_t st) {
+  if (B < 1 || P < 1 || E < 2 || (E & 1)) return -3;
+  if (misaligned(pe, 4) || misaligned(cls, 8) || misaligned(pos, 8) || misaligned(out, 4)) return -4;
+  const int tokens = B * (P + 1);
+  vit_tokens_kernel<<<(tokens + 7) / 8, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(pe), cls, pos,
+                                                      reinterpret_cast<__nv_bfloat16*>(out), B, P, E);
+  return check_launch();
+}
+// x bf16 rows at pitch ldx (elements), y bf16 [rows][D]; D even, ldx >= D and even
+int slb_ln_rows_fwd(const void* x, long long ldx, const float* gamma, const float* beta, void* y, int rows, int D, float eps,
+                    cudaStream_t st) {
+  if (rows < 1 || D < 2 || (D & 1)) return -3;
+  if (ldx < D || (ldx & 1) || misaligned(x, 4) || misaligned(y, 4) || misaligned(gamma, 8) || misaligned(beta, 8)) return -4;
+  ln_rows_fwd_kernel<<<(rows + 7) / 8, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), ldx, gamma, beta,
+                                                     reinterpret_cast<__nv_bfloat16*>(y), rows, D, eps);
+  return check_launch();
+}
+
 int slb_preload_transformer() {
   cudaFuncAttributes a;
   int bad = 0;
@@ -739,6 +846,9 @@ int slb_preload_transformer() {
   bad |= cudaFuncGetAttributes(&a, dropout_bf16_kernel) != cudaSuccess;
   bad |= cudaFuncGetAttributes(&a, embed3_fwd_kernel) != cudaSuccess;
   bad |= cudaFuncGetAttributes(&a, embed3_bwd_kernel) != cudaSuccess;
+  bad |= cudaFuncGetAttributes(&a, patch_rows_kernel) != cudaSuccess;
+  bad |= cudaFuncGetAttributes(&a, vit_tokens_kernel) != cudaSuccess;
+  bad |= cudaFuncGetAttributes(&a, ln_rows_fwd_kernel) != cudaSuccess;
   return bad ? -1 : 0;
 }
 

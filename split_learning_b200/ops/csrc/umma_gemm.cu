@@ -541,7 +541,13 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = static
             for (int j = 0; j < 32; ++j)
               if (col0 + j < p.N) atomicAdd(o + static_cast<long long>(col0 + j) * p.ldo, __uint_as_float(v[j]));
           }
-        } else {  // EPI_F32_STORE
+        } else {  // EPI_F32_STORE (MODE_GEMM with a bias: fp32 logits = acc + bias, slb_gemm_bf16_bias_f32)
+          if constexpr (MODE == MODE_GEMM) {
+            if (p.bias != nullptr) {
+#pragma unroll
+              for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + s_bias[c + j]);
+            }
+          }
           if (row_store) {
             float* o = reinterpret_cast<float*>(p.out) + row_off + col0;
             if (col0 + 32 <= p.N && vec16_ok<MODE>(o)) {
@@ -1071,6 +1077,26 @@ int slb_gemm_bf16_act(const void* A, const void* Bm, void* out, int M, int N, in
   p.a_mn = a_mn; p.b_mn = b_mn; p.epi = EPI_BF16; p.out = out; p.ldo = ldo;
   p.bias = bias; p.act = act; p.aux_out = reinterpret_cast<__nv_bfloat16*>(aux);
   p.residual = reinterpret_cast<const __nv_bfloat16*>(residual);
+  dim3 grid((M + 127) / 128, (N + block_n - 1) / block_n, 1);
+  return dispatch_bn<MODE_GEMM>(block_n, 0, ta, tbm, p, grid, st);
+}
+
+// Classifier head with fp32 output: out_f32[M][ldo] = A[M][K] * B[N][K]^T + bias (both operands K-major, plain store,
+// no split-K).  The logits go straight to the loss / accuracy kernel without a bf16 rounding or a cast.
+int slb_gemm_bf16_bias_f32(const void* A, const void* Bm, float* out, int M, int N, int K, long long lda, long long ldb,
+                           long long ldo, int block_n, const float* bias, cudaStream_t st) {
+  if (block_n != 32 && block_n != 64 && block_n != 128 && block_n != 256) return -3;
+  if (M < 1 || N < 1 || K < 1 || K % 8 || lda < K || ldb < K || ldo < N || (lda | ldb) & 7) return -4;
+  if (!A || !Bm || !out || !bias || (reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Bm)) & 15 ||
+      (reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(bias)) & 3)
+    return -5;
+  CUtensorMap ta, tbm;
+  int r;
+  if ((r = tmap_2d(&ta, A, K, M, lda, 64, 128))) return r;
+  if ((r = tmap_2d(&tbm, Bm, K, N, ldb, 64, block_n))) return r;
+  GemmParams p = {};
+  p.M = M; p.N = N; p.k_iters = (K + 63) / 64; p.k_split = 1;
+  p.a_mn = 0; p.b_mn = 0; p.epi = EPI_F32_STORE; p.out = out; p.ldo = ldo; p.bias = bias;
   dim3 grid((M + 127) / 128, (N + block_n - 1) / block_n, 1);
   return dispatch_bn<MODE_GEMM>(block_n, 0, ta, tbm, p, grid, st);
 }

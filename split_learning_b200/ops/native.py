@@ -599,6 +599,35 @@ def gemm_f32(a, b, out, M, N, K, a_mn=False, b_mn=False, lda=None, ldb=None, ldo
                                _stream()), "gemm_f32")
 
 
+def gemm_bias_f32(a, b, out, bias, M, N, K, lda=None, ldb=None, ldo=None, block_n=None):
+    """out_fp32[M, N] = A B^T + bias, plain store: A [M, K] and B [N, K] bf16, both K-major (a classifier head whose logits
+    feed ``eval_metrics`` without a bf16 rounding).  ``lda`` may exceed K (rows picked out of a wider tensor)."""
+    lda = lda if lda is not None else K
+    ldb = ldb if ldb is not None else K
+    ldo = ldo if ldo is not None else N
+    bn = block_n if block_n is not None else _gemm_bn(N, M)
+    _check(lib().slb_gemm_bf16_bias_f32(_p(a), _p(b), _p(out), c_int(M), c_int(N), c_int(K), c_longlong(lda), c_longlong(ldb),
+                                        c_longlong(ldo), c_int(bn), _p(bias), _stream()), "gemm_bias_f32")
+
+
+def patch_rows(x, out, p: int):
+    """x fp32 [B, C, H, W] -> out bf16 [B * (H/p) * (W/p), C * p * p]: the unfolded patches of a Conv2d(kernel = stride = p),
+    row (b, gy, gx), column (c, py, px)."""
+    B, C, H, W = x.shape
+    _check(lib().slb_patch_rows(_p(x), _p(out), c_int(B), c_int(C), c_int(H), c_int(W), c_int(p), _stream()), "patch_rows")
+
+
+def vit_tokens(pe, cls, pos, out, B: int, P: int, E: int):
+    """out bf16 [B, P+1, E] = cat(cls, pe [B, P, E]) + pos [P+1, E] (fp32 adds, one bf16 rounding)."""
+    _check(lib().slb_vit_tokens(_p(pe), _p(cls), _p(pos), _p(out), c_int(B), c_int(P), c_int(E), _stream()), "vit_tokens")
+
+
+def ln_rows_fwd(x, ldx: int, gamma, beta, y, rows: int, D: int, eps: float):
+    """y bf16 [rows, D] = LayerNorm of the rows of ``x`` at pitch ``ldx`` elements (inference: no statistics kept)."""
+    _check(lib().slb_ln_rows_fwd(_p(x), c_longlong(ldx), _p(gamma), _p(beta), _p(y), c_int(rows), c_int(D), c_float(eps),
+                                 _stream()), "ln_rows_fwd")
+
+
 def attn_fwd(q, k, v, ldq, ldk, ldv, q_col, k_col, v_col, out, ldo, lse, key_bias, B, S, H, Dh, p_drop=0.0, seed=0,
              seed_ofs=None):
     _check(lib().slb_attn_fwd(_p(q), _p(k), _p(v), c_longlong(ldq), c_longlong(ldk), c_longlong(ldv), c_int(q_col),

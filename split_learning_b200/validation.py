@@ -8,8 +8,9 @@ hook DCSL uses to keep its AMQP heartbeat alive (other/DCSL/src/Validation.py:48
 lets the broker thread breathe / watchdogs tick.
 
 ``native`` (``b200.native-validation``) selects the backend: ``false`` (default) the torch modules above; ``true`` the
-native eval plan (``train/b200_eval.py``) on the test split resident in HBM, an error where there is none; ``auto`` native
-where supported, torch otherwise with one log line giving the reason.  Metrics carry ``val_backend``.
+native eval plan on the test split resident in HBM — ``train/b200_eval.py`` for VGG16_CIFAR10, ``train/token_eval.py``
+for ViT_CIFAR10, BERT_AGNEWS and BERT_EMOTION — an error where there is none; ``auto`` native where supported, torch
+otherwise with one log line giving the reason.  Metrics carry ``val_backend``.
 """
 from __future__ import annotations
 
@@ -23,7 +24,7 @@ import torch.nn as nn
 from .data import data_loader
 from .models import get_model_class
 
-_NATIVE: Dict[Tuple, Any] = {}          # (model, data, device, synthetic) -> (NativeEvaluator, resident test split)
+_NATIVE: Dict[Tuple, Any] = {}          # (model, data, device, synthetic) -> (evaluator, resident test split)
 
 
 @torch.no_grad()
@@ -68,6 +69,11 @@ def native_unsupported_reason(klass, data_name: str, device) -> Optional[str]:
     dev = torch.device(device)
     if dev.type != "cuda" or not torch.cuda.is_available():
         return "no CUDA device"
+    from .train.token_eval import token_eval_supported
+    if token_eval_supported(klass):
+        if str(data_name).upper() != klass.DATA_NAME:
+            return f"no resident test split for {data_name}"
+        return None
     if str(data_name).upper() != "CIFAR10":
         return f"no resident test split for {data_name}"
     from .train.b200_eval import native_eval_supported
@@ -79,13 +85,15 @@ def native_unsupported_reason(klass, data_name: str, device) -> Optional[str]:
 def _native_evaluate(klass, model_name, data_name, state_dict_full, device, pump, synthetic) -> Dict[str, float]:
     from .data import resident_test_loader
     from .train.b200_eval import NativeEvaluator
+    from .train.token_eval import NativeTokenEvaluator, token_eval_supported
     dev = torch.device(device)
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
     key = (model_name, str(data_name).upper(), str(dev), synthetic)
     hit = _NATIVE.get(key)
     if hit is None:
-        hit = _NATIVE[key] = (NativeEvaluator(klass, state_dict_full, dev), resident_test_loader(data_name, dev, synthetic))
+        cls = NativeTokenEvaluator if token_eval_supported(klass) else NativeEvaluator
+        hit = _NATIVE[key] = (cls(klass, state_dict_full, dev), resident_test_loader(data_name, dev, synthetic))
     else:
         hit[0].load_state_dict(state_dict_full)
     evaluator, source = hit
