@@ -150,7 +150,7 @@ conv_bn_act_p2p_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     uint32_t phase = 0;
     for (int j = 0; j < my_tiles; ++j) {
       float acc[BLOCK_N / 2];
-      wg_mainloop<T, BLOCK_N>(smem, nullptr, L::STAGE_BYTES, L::A_BYTES, L::STAGES, full_bar, empty_bar, k_iters, 0, 0, acc,
+      wg_mainloop<T, BLOCK_N>(smem, L::STAGE_BYTES, L::A_BYTES, L::STAGES, full_bar, empty_bar, k_iters, 0, 0, acc,
                               stage, phase);
       if (j == my_tiles - 1) asm volatile("bar.sync 2, 256;" ::: "memory");   // no MMA reads the ring any more
       wg_store_acc<BLOCK_N>(tile_acc(j) + (threadIdx.x >> 7) * 64 * L::ACC_LD, L::ACC_LD, acc);

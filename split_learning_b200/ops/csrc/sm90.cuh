@@ -204,53 +204,95 @@ template <> struct OperandTraits<float> {
   static constexpr bool TF32 = true;
 };
 
-// wgmma reads tf32 operands K-major only.  An fp32 operand stored MN-major (loaded by TMA without swizzle: groups of
-// 32 M/N elements x 32 k-rows of 128 B, 4 KB apart) is transposed by the 256 consumer threads into a K-major
-// 128B-swizzled tile of `rows` rows before the MMAs read it.
-__device__ __forceinline__ void transpose_tf32_kmajor(uint8_t* dst, const uint8_t* src, int rows) {
-  const float* s = reinterpret_cast<const float*>(src);
-  for (int i = threadIdx.x; i < rows * 8; i += 256) {
-    const int r = i & (rows - 1), c = i / rows;                    // row r, 16-byte chunk c (k = 4c .. 4c + 3)
-    const float* col = s + (r >> 5) * 1024 + (4 * c) * 32 + (r & 31);
-    *reinterpret_cast<float4*>(dst + r * 128 + ((c ^ (r & 7)) << 4)) = make_float4(col[0], col[32], col[64], col[96]);
+// wgmma reads tf32 operands K-major only.  An fp32 operand stored MN-major is loaded by TMA without swizzle, as groups
+// of 32 M/N elements x 32 k-rows of 128 B (4 KB each).  Group g holds exactly the bytes that rows [32g, 32g + 32) of a
+// K-major 128B-swizzled tile occupy, so the 256 consumer threads transpose the stage in place, group by group: each
+// thread reads one 16-byte chunk (k = 4c .. 4c + 3 of row r) of up to four groups into registers, all threads meet at a
+// barrier, then write them back K-major.  Reads (32 consecutive floats per warp) and 16-byte writes (8 distinct chunks of
+// 8 rows per quarter-warp) are free of bank conflicts.  `groups` counts the consecutive groups from `tile`.
+__device__ __forceinline__ void transpose_tf32_inplace(uint8_t* tile, int groups) {
+  const int r = threadIdx.x & 31, c = threadIdx.x >> 5;
+  uint8_t* dst = tile + r * 128 + ((c ^ (r & 7)) << 4);
+  const float* src = reinterpret_cast<const float*>(tile) + 4 * c * 32 + r;
+  for (int g0 = 0; g0 < groups; g0 += 4) {
+    float4 v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float* col = src + (g0 + j) * 1024;
+      if (g0 + j < groups) v[j] = make_float4(col[0], col[32], col[64], col[96]);
+    }
+    asm volatile("bar.sync 2, 256;" ::: "memory");                 // these groups are read out before any is rewritten
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (g0 + j < groups) *reinterpret_cast<float4*>(dst + (g0 + j) * 4096) = v[j];
   }
 }
 
 // Consumer side of a TMA -> wgmma ring, run by two warpgroups (threads 0..255) that own rows [0, 64) and [64, 128) of
 // a 128 x BLOCK_N tile.  Stage s: A (128 x KE, at smem + s * stage_bytes) then B (BLOCK_N x KE, a_bytes further); K-major
 // operands are 128-byte swizzled rows, bf16 MN-major operands are 64-wide groups of KE k-rows.  empty_bar[s] expects one
-// arrival per warpgroup.  `stg` (fp32 only): 128 x 128 B + BLOCK_N x 128 B of K-major staging for MN-major operands.
+// arrival per warpgroup.
+//
+// tf32 with an MN-major operand: every stage is transposed in place (transpose_tf32_inplace) one K step ahead, while
+// the previous step's MMAs run.  Step i's MMAs read stage i only; the transpose of stage i + 1 touches no other stage.
+// A stage goes back to the producer once the MMAs that read it have retired (wgmma_wait<1> one step later), and it is
+// only refilled after that, so with >= 3 stages the stage being transposed is never one the tensor cores still read.
 template <typename T, int BLOCK_N>
-__device__ __forceinline__ void wg_mainloop(uint8_t* smem, uint8_t* stg, int stage_bytes, int a_bytes, int stages,
+__device__ __forceinline__ void wg_mainloop(uint8_t* smem, int stage_bytes, int a_bytes, int stages,
                                             uint64_t* full_bar, uint64_t* empty_bar, int iters, int a_mn, int b_mn,
                                             float (&acc)[BLOCK_N / 2], int& stage, uint32_t& phase) {
   using OT = OperandTraits<T>;
   constexpr int GROUP_BYTES = OT::KE * 128;
   const uint32_t half = static_cast<uint32_t>(threadIdx.x >> 7) * 8192;   // 64 rows K-major == one MN-major group
-  const bool transpose = OT::TF32 && (a_mn || b_mn);
   int prev = -1;
+  if constexpr (OT::TF32) {
+    if (a_mn || b_mn) {
+      const int groups = (a_mn ? 4 : 0) + (b_mn ? BLOCK_N / 32 : 0);   // A is 4 groups; B follows A in the stage
+      const int goff = a_mn ? 0 : a_bytes;
+      if (iters > 0) {
+        mbar_wait(&full_bar[stage], phase);
+        transpose_tf32_inplace(smem + stage * stage_bytes + goff, groups);
+        fence_proxy_async();
+        asm volatile("bar.sync 2, 256;" ::: "memory");
+      }
+      for (int it = 0; it < iters; ++it) {
+        const uint32_t a_base = smem_u32(smem + stage * stage_bytes), b_base = a_base + a_bytes;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)                                 // both operands are K-major now
+          Wgmma<T, BLOCK_N>::mma(acc, wg_desc_sw128(a_base + half + k * 32, 16, 1024), wg_desc_sw128(b_base + k * 32, 16, 1024),
+                                 (it | k) != 0 ? 1u : 0u, 0, 0);
+        wgmma_commit();
+        int next = stage + 1;
+        uint32_t next_phase = phase;
+        if (next == stages) { next = 0; next_phase ^= 1; }
+        if (it + 1 < iters) {                                       // overlaps this step's MMAs
+          mbar_wait(&full_bar[next], next_phase);
+          transpose_tf32_inplace(smem + next * stage_bytes + goff, groups);
+          fence_proxy_async();                                      // generic-proxy writes -> the wgmma reads
+        }
+        wgmma_wait<1>();                                            // the previous stage's MMAs have retired
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        stage = next;
+        phase = next_phase;
+        asm volatile("bar.sync 2, 256;" ::: "memory");             // the next stage is K-major in both warpgroups' view
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      return;
+    }
+  }
   for (int it = 0; it < iters; ++it) {
     mbar_wait(&full_bar[stage], phase);
-    uint8_t* st = smem + stage * stage_bytes;
-    uint32_t a_base = smem_u32(st), b_base = a_base + a_bytes;
-    int amn = a_mn, bmn = b_mn;
-    if (transpose) {
-      wgmma_wait<0>();
-      asm volatile("bar.sync 2, 256;" ::: "memory");               // both warpgroups are done with the staging tiles
-      if (a_mn) transpose_tf32_kmajor(stg, st, 128);
-      if (b_mn) transpose_tf32_kmajor(stg + 128 * 128, st + a_bytes, BLOCK_N);
-      fence_proxy_async();
-      asm volatile("bar.sync 2, 256;" ::: "memory");
-      if (a_mn) { a_base = smem_u32(stg); amn = 0; }
-      if (b_mn) { b_base = smem_u32(stg) + 128 * 128; bmn = 0; }
-    }
+    const uint32_t a_base = smem_u32(smem + stage * stage_bytes), b_base = a_base + a_bytes;
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const uint64_t da = amn ? wg_desc_sw128(a_base + half + k * 2048, GROUP_BYTES, 1024)
-                              : wg_desc_sw128(a_base + half + k * 32, 16, 1024);
-      const uint64_t db = bmn ? wg_desc_sw128(b_base + k * 2048, GROUP_BYTES, 1024) : wg_desc_sw128(b_base + k * 32, 16, 1024);
-      Wgmma<T, BLOCK_N>::mma(acc, da, db, (it | k) != 0 ? 1u : 0u, amn, bmn);
+      const uint64_t da = a_mn ? wg_desc_sw128(a_base + half + k * 2048, GROUP_BYTES, 1024)
+                               : wg_desc_sw128(a_base + half + k * 32, 16, 1024);
+      const uint64_t db = b_mn ? wg_desc_sw128(b_base + k * 2048, GROUP_BYTES, 1024) : wg_desc_sw128(b_base + k * 32, 16, 1024);
+      Wgmma<T, BLOCK_N>::mma(acc, da, db, (it | k) != 0 ? 1u : 0u, a_mn, b_mn);
     }
     wgmma_commit();
     wgmma_wait<1>();                                                // the previous stage's MMAs have retired

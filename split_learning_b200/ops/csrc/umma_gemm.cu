@@ -97,10 +97,11 @@ struct SmemLayout {
   static constexpr int A_BYTES = 128 * 128;      // 16 KB
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGING = OperandTraits<T>::TF32 ? STAGE_BYTES : 0;   // K-major copies of MN-major fp32 operands
-  static constexpr int STAGES_FIT = (196 * 1024 - STAGING) / STAGE_BYTES;
+  static constexpr int STAGES_FIT = 196 * 1024 / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT < 6 ? STAGES_FIT : 6;
-  static constexpr int TILE_BYTES = STAGES * STAGE_BYTES + STAGING;
+  // tf32 MN-major operands are transposed in place one stage ahead of the MMAs (sm90.cuh wg_mainloop)
+  static_assert(STAGES >= 3, "the in-place tf32 transpose needs a third stage");
+  static constexpr int TILE_BYTES = STAGES * STAGE_BYTES;
   // once the MMAs are done the ring holds the epilogue's transpose tiles [0, 17 KB) and the fp32 accumulator tile
   static constexpr int ACC_OFF = 17 * 1024;
   static constexpr int ACC_LD = BLOCK_N + 4;     // row pitch in floats: 16-byte row reads without bank conflicts
@@ -396,8 +397,8 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       float acc[BLOCK_N / 2];
       int stage = 0;
       uint32_t phase = 0;
-      wg_mainloop<T, BLOCK_N>(smem, smem + L::STAGES * L::STAGE_BYTES, L::STAGE_BYTES, L::A_BYTES, L::STAGES, full_bar,
-                              empty_bar, my_iters, p.a_mn, p.b_mn, acc, stage, phase);
+      wg_mainloop<T, BLOCK_N>(smem, L::STAGE_BYTES, L::A_BYTES, L::STAGES, full_bar, empty_bar, my_iters, p.a_mn, p.b_mn,
+                              acc, stage, phase);
       if (et == 0) SLB_STAMP(6);                               // accumulator complete
       asm volatile("bar.sync 2, 256;" ::: "memory");           // no MMA reads the ring any more
       wg_store_acc<BLOCK_N>(s_acc + (threadIdx.x >> 7) * 64 * L::ACC_LD, L::ACC_LD, acc);
@@ -589,9 +590,10 @@ _Pragma("unroll") for (int j = 0; j < 32; ++j) if (col0 + j < p.N) o[j] = __uint
 #pragma unroll
             for (int j = 0; j < 32; ++j) f[j] = 0.f;
             if (row_ok) {
-              // +0 plus the slices in slice order with add.rn.ftz: the arithmetic of red.global.add.f32 into a zeroed buffer
+              // +0 plus the slices in slice order with add.rn.ftz: the arithmetic of red.global.add.f32 into a zeroed buffer.
+              // Unrolled by four slices so that 32 independent L2 loads are in flight, not 8 per dependent round trip.
               const float4* a4 = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.out) + row_off + col0);
-#pragma unroll 1
+#pragma unroll 4
               for (int zz = 0; zz < static_cast<int>(gridDim.z); ++zz) {
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
@@ -701,7 +703,7 @@ static int make_tmap(CUtensorMap* m, const void* base, int rank, const uint64_t*
     es[i] = 1;
     if (i > 0) gstr[i - 1] = strides_bytes[i];
   }
-  // MN-major fp32 (tf32) operands land unswizzled and are transposed in shared memory (sm90.cuh transpose_tf32_kmajor)
+  // MN-major fp32 (tf32) operands land unswizzled and are transposed in shared memory (sm90.cuh transpose_tf32_inplace)
   const CUtensorMapSwizzle sw = (dtype == 1 && mn_major) ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B;
   CUresult r = enc(m, tmap_dtype(dtype), rank, const_cast<void*>(base), gdim, gstr, bx, es,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,

@@ -168,6 +168,32 @@ def conv8_dgrad_cut_head(iters):
             "link_bytes": dx.numel() * ISZ()}
 
 
+def _conv_bwd(op, B, H, W, Cin, Cout, iters):
+    """Input or weight gradient of one conv at the executor's tiling: conv_tiling(flip=1) with in-kernel split-K
+    finalisation for dX, the automatic split for dW (which zeroes dW before every launch, as the executor does)."""
+    x, w, _ = conv_case(B, H, W, Cin, Cout)
+    dy = bf(torch.randn(B, H, W, Cout, device="cuda"))
+    flops = 2.0 * B * H * W * Cout * 9 * Cin
+    if op == "dgrad":
+        dx = torch.empty(B, H, W, Cin, device="cuda", dtype=ADT())
+        bn_, ks = N.conv_tiling(B * H * W, Cin, Cout, flip=1, ke=32 if PREC == "tf32" else 64)
+        acc = torch.empty(N.conv_partial_floats(B * H * W, Cin, ks), device="cuda") if ks > 1 else None
+        ctr = torch.zeros(4096, device="cuda", dtype=torch.int32)
+        med, best = timeit(lambda: N.conv3x3_dgrad(dy, w, dx, acc=acc, counters=ctr), iters)
+        return {"us": med, "best_us": best, "flops": flops, "bytes": (dy.numel() + w.numel() + dx.numel()) * ISZ(),
+                "tiling": [bn_, ks]}
+    dw = torch.zeros(Cout, 3, 3, Cin, device="cuda")
+    med, best = timeit(lambda: N.conv3x3_wgrad(x, dy, dw), iters, setup=dw.zero_)
+    return {"us": med, "best_us": best, "flops": flops, "bytes": (x.numel() + dy.numel()) * ISZ() + dw.numel() * 4}
+
+
+# every conv of VGG16/CIFAR10 below the cut at layer 7 (stage 2), and stage 1's 64 -> 64 at 32 x 32
+for _B, _H, _ci, _co in [(32, 32, 64, 64), (32, 16, 64, 128), (32, 16, 128, 128), (32, 8, 128, 256), (32, 8, 256, 256),
+                         (32, 4, 256, 512), (32, 4, 512, 512), (32, 2, 512, 512)]:
+    for _op in ("dgrad", "wgrad"):
+        CASES[f"{_op}_{_H}x{_H}_{_ci}_{_co}"] = (lambda op, s: lambda iters: _conv_bwd(op, *s, iters))(_op, (_B, _H, _H, _ci, _co))
+
+
 def _fused(B, H, W, Cin, Cout, relu, pool, iters):
     x, w, bias = conv_case(B, H, W, Cin, Cout)
     gamma, beta = torch.ones(Cout, device="cuda"), torch.zeros(Cout, device="cuda")
