@@ -1,4 +1,4 @@
-"""GPU-resident image loader (``b200.gpu-loader: true``).
+"""GPU-resident training loaders (``b200.gpu-loader: true``): images and Speech Commands features.
 
 The reference builds every microbatch on the host: PIL crop / flip / ToTensor / Normalize per sample in a
 ``DataLoader`` (src/dataset/dataloader.py:61-84), then ``.to(device)``.  CIFAR-10 is 150 MB of uint8 — it fits in a
@@ -6,6 +6,10 @@ corner of an H100's 80 GB of HBM — so here the selected training subset lives 
 (``image_batch_kernel``): gather by shuffled index, RandomCrop(32, padding 4), RandomHorizontalFlip, /255, Normalize,
 written as the fp32 NCHW stage input.  No host work and no H2D copy per step; the iterator yields device tensors, which
 every executor and the device data plane accept as they are.
+
+Speech Commands (KWT) is held as its MFCC features: the host reads each ``.wav`` once, ``mfcc_kernel`` turns the clips into
+[40, 98] features in fp64 with the tables of ``speechcommands.mfcc()`` (the same values the host loader computes per
+``__getitem__``), and each microbatch is one gather (``GpuFeatureLoader``, ``feature_batch_kernel``).
 """
 from __future__ import annotations
 
@@ -62,6 +66,57 @@ class GpuImageLoader:
                  else torch.arange(self.n, device=self.device))
         for k in range(len(self)):
             yield self.batch(order[k * self.batch_size:(k + 1) * self.batch_size])
+
+
+class GpuFeatureLoader:
+    """Iterable of (x [B, *sample] fp32, y [B] int64) device tensors gathered from a resident fp32 split, one
+    ``feature_batch`` launch per microbatch; ``len()`` = microbatches per epoch, a fresh permutation per epoch drawn on the
+    device generator, the short batch last.  Speech Commands: the [N, 40, 98] MFCC features (``speech_gpu_loader``)."""
+
+    def __init__(self, features: torch.Tensor, labels: torch.Tensor, batch_size: int, device, shuffle: bool = True,
+                 seed: Optional[int] = None):
+        if features.dtype != torch.float32 or features.dim() < 2:
+            raise ValueError("features must be fp32 [N, ...]")
+        self.device = torch.device(device)
+        self.features = features.to(self.device).contiguous()
+        self.labels = labels.long().to(self.device).contiguous()
+        self.n = self.features.shape[0]
+        self.batch_size, self.shuffle = int(batch_size), shuffle
+        self.gen = torch.Generator(device=self.device)
+        self.gen.manual_seed(int(seed) if seed is not None else torch.initial_seed() & 0x7FFFFFFF)
+        N.require()
+
+    def __len__(self):
+        return (self.n + self.batch_size - 1) // self.batch_size
+
+    def batch(self, idx: torch.Tensor):
+        b = idx.numel()
+        x = torch.empty((b,) + tuple(self.features.shape[1:]), dtype=torch.float32, device=self.device)
+        y = torch.empty(b, dtype=torch.long, device=self.device)
+        N.feature_batch(self.features, self.labels, idx.contiguous(), x, y)
+        return x, y
+
+    def __iter__(self):
+        order = (torch.randperm(self.n, device=self.device, generator=self.gen) if self.shuffle
+                 else torch.arange(self.n, device=self.device))
+        for k in range(len(self)):
+            yield self.batch(order[k * self.batch_size:(k + 1) * self.batch_size])
+
+
+def mfcc_tables(device):
+    """``speechcommands.mfcc_tables()`` as fp64 device tensors (the kernel's window, filterbank, DCT and twiddles)."""
+    from .speechcommands import mfcc_tables as host_tables
+    return {k: torch.from_numpy(v).to(device=device, dtype=torch.float64).contiguous() for k, v in host_tables().items()}
+
+
+def mfcc_features(waves: torch.Tensor, valid: torch.Tensor, tables: dict, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 [n, 40, 98] MFCC features of fp32 waveforms [n, L] (already padded or truncated to L) on the GPU, one
+    ``mfcc`` launch; clips with ``valid == 0`` get zeros, as ``SpeechCommandsDataset`` gives unreadable files."""
+    from .speechcommands import FRAMES, HOP, LOG_FLOOR, N_MFCC, PREEMPH
+    if out is None:
+        out = torch.empty(waves.shape[0], N_MFCC, FRAMES, dtype=torch.float32, device=waves.device)
+    N.mfcc(waves, valid, out, tables["window"], tables["fb"], tables["dct"], tables["twiddle"], HOP, PREEMPH, LOG_FLOOR)
+    return out
 
 
 class ResidentBatches:

@@ -9,6 +9,8 @@ Real datasets follow the reference's recipes (src/dataset/dataloader.py):
 They need files under ``./data`` (no network here).  When the files are missing, or
 ``synthetic=True`` / ``SLB200_SYNTHETIC=1``, a ``SyntheticDataset`` with the same tensor
 shapes, dtypes and per-label counts is used instead (what ``bench.py`` uses).
+With ``gpu_loader=True`` on a CUDA device, CIFAR10 / MNIST / SPEECHCOMMANDS training subsets are held in HBM instead
+(``data/gpu_loader.py``).
 """
 from __future__ import annotations
 
@@ -217,6 +219,66 @@ def gpu_image_loader(name: str, batch_size: int, distribution: Sequence[int], de
     return GpuImageLoader(images, y, batch_size, device, mean, std, augment=(name == "CIFAR10"), seed=seed)
 
 
+SPEECH_CHUNK = 2048      # clips per upload + ``mfcc`` launch while a resident Speech Commands split is built (~130 MB)
+
+
+def speech_features(paths: Sequence[str], device, chunk: int = SPEECH_CHUNK, timing: Optional[dict] = None) -> torch.Tensor:
+    """fp32 [len(paths), 40, 98] device tensor of the MFCC features ``SpeechCommandsDataset.__getitem__`` gives these files:
+    the host reads and converts each file as it does (``read_wave``), pads or truncates it to L = 15 920 samples, and
+    every ``chunk`` clips go to the GPU for one ``mfcc`` launch.  Only the features stay resident; unreadable files get zero
+    rows.  ``timing``: accumulates ``host_s`` (file reads) and ``mfcc_ms`` (kernel time, CUDA events)."""
+    import time
+
+    import numpy as np
+    from .gpu_loader import mfcc_features, mfcc_tables
+    from .speechcommands import FRAMES, HOP, N_MFCC, WIN, read_wave
+    dev = torch.device(device)
+    L = WIN + HOP * (FRAMES - 1)
+    tables = mfcc_tables(dev)
+    feats = torch.empty(len(paths), N_MFCC, FRAMES, dtype=torch.float32, device=dev)
+    for lo in range(0, len(paths), chunk):
+        part = paths[lo:lo + chunk]
+        t0 = time.perf_counter()
+        waves = np.zeros((len(part), L), dtype=np.float32)
+        valid = np.ones(len(part), dtype=np.uint8)
+        for r, path in enumerate(part):
+            try:
+                w = read_wave(path)[:L]
+            except Exception:
+                valid[r] = 0
+                continue
+            waves[r, :w.size] = w
+        if timing is not None:
+            timing["host_s"] = timing.get("host_s", 0.0) + time.perf_counter() - t0
+        wd, vd = torch.from_numpy(waves).to(dev), torch.from_numpy(valid).to(dev)
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if timing is not None else None
+        if ev:
+            ev[0].record()
+        mfcc_features(wd, vd, tables, out=feats[lo:lo + len(part)])
+        if ev:
+            ev[1].record()
+            ev[1].synchronize()
+            timing["mfcc_ms"] = timing.get("mfcc_ms", 0.0) + ev[0].elapsed_time(ev[1])
+    return feats
+
+
+def speech_gpu_loader(batch_size: int, distribution: Sequence[int], device, synthetic: bool, root: str = "./data",
+                      seed: int = 0):
+    """Speech Commands training loader whose split lives on the GPU as MFCC features (``GpuFeatureLoader``): real data takes
+    the sample list and per-label subset of ``_speechcommands`` and computes the features once (``speech_features``);
+    synthetic data uploads the samples of the host synthetic loader."""
+    from .gpu_loader import GpuFeatureLoader
+    if synthetic:
+        ds = SyntheticDataset("SPEECHCOMMANDS", distribution, seed=seed)
+        return GpuFeatureLoader(ds.data, ds.labels, batch_size, device, seed=seed)
+    from .speechcommands import CLASSES, SpeechCommandsDataset
+    ds = SpeechCommandsDataset(root=root, subset="training")
+    labels = [CLASSES.index(name) for _, name in ds.samples]
+    pick = _select_by_label(labels, distribution)
+    feats = speech_features([ds.samples[i][0] for i in pick], device)
+    return GpuFeatureLoader(feats, torch.tensor([labels[i] for i in pick], dtype=torch.long), batch_size, device, seed=seed)
+
+
 _WARNED: set = set()
 
 
@@ -276,6 +338,9 @@ def data_loader(data_name: Optional[str] = None, batch_size: Optional[int] = Non
     if (gpu_loader and train and name in ("CIFAR10", "MNIST") and device is not None and torch.device(device).type == "cuda"
             and distribution is not None and len(distribution) > 0):
         return gpu_image_loader(name, int(batch_size), distribution, device, bool(synthetic), root, seed)
+    if (gpu_loader and train and name == "SPEECHCOMMANDS" and device is not None and torch.device(device).type == "cuda"
+            and distribution is not None and len(distribution) > 0):
+        return speech_gpu_loader(int(batch_size), distribution, device, bool(synthetic), root, seed)
     if synthetic or name not in _REAL:
         shape, dtype, ncls, test_bs = DATASET_SHAPES[name]
         if distribution is None or len(distribution) == 0:

@@ -1,9 +1,13 @@
 """Speech Commands (10-class subset) with a NumPy MFCC front-end.
 
-Same feature recipe as reference src/dataset/SPEECHCOMMANDS.py:11-47 (pre-emphasis 0.97,
-25 ms Hamming frames / 10 ms hop at 16 kHz, 512-point rFFT power spectrum, 40 mel filters,
-log, DCT-II → 40 coefficients, 98 frames), written here as vectorised framing + one matmul
-per stage.  Unreadable files become zeros (:116-118).
+The shape of the reference's recipe (src/dataset/SPEECHCOMMANDS.py:11-47: pre-emphasis 0.97,
+25 ms Hamming frames / 10 ms hop at 16 kHz, power spectrum, 40 mel filters, log, DCT → 40
+coefficients, 98 frames), written here as vectorised framing + one matmul per stage.  It is not
+the reference's exact recipe (a known open issue, see PARITY.md): the reference frames with
+n_fft = 480 directly where this zero-pads a 400-sample window to 512, takes 20·log10 with exact
+zeros replaced by eps where this takes ln(max(·, 1e-10)), and uses scipy's orthonormal DCT.
+Unreadable files become zeros (:116-118).  ``b200.gpu-loader`` computes the same features on
+the GPU from ``mfcc_tables()`` (data/gpu_loader.py).
 """
 from __future__ import annotations
 
@@ -16,6 +20,7 @@ from torch.utils.data import Dataset
 
 CLASSES = ["yes", "no", "up", "down", "left", "right", "on", "off", "stop", "go"]
 SAMPLE_RATE, N_MFCC, N_MELS, N_FFT, WIN, HOP, FRAMES = 16000, 40, 40, 512, 400, 160, 98
+PREEMPH, LOG_FLOOR = 0.97, 1e-10
 
 
 def _mel_filterbank(n_mels=N_MELS, n_fft=N_FFT, sr=SAMPLE_RATE) -> np.ndarray:
@@ -49,12 +54,28 @@ def mfcc(wave: np.ndarray) -> np.ndarray:
     w = np.asarray(wave, dtype=np.float64).ravel()
     need = WIN + HOP * (FRAMES - 1)
     w = np.pad(w, (0, max(0, need - w.size)))[:need]
-    w = np.append(w[0], w[1:] - 0.97 * w[:-1])
+    w = np.append(w[0], w[1:] - PREEMPH * w[:-1])
     idx = np.arange(WIN)[None, :] + HOP * np.arange(FRAMES)[:, None]
     frames = w[idx] * _WINDOW
     power = (np.abs(np.fft.rfft(frames, N_FFT)) ** 2) / N_FFT
-    mel = np.log(np.maximum(power @ _FB.T, 1e-10))
+    mel = np.log(np.maximum(power @ _FB.T, LOG_FLOOR))
     return (mel @ _DCT.T).T.astype(np.float32)
+
+
+def mfcc_tables():
+    """The fp64 tables of ``mfcc()`` as the GPU kernel takes them (``ops.native.mfcc``): the window, the mel filterbank, the
+    DCT matrix, and the (cos, sin) of 2 pi j / N_FFT for j < N_FFT, whose entry (k * t) mod N_FFT is the twiddle of bin k
+    at sample t."""
+    j = np.arange(N_FFT) * (2.0 * np.pi / N_FFT)
+    return {"window": _WINDOW, "fb": _FB, "dct": _DCT, "twiddle": np.stack([np.cos(j), np.sin(j)], axis=1)}
+
+
+def read_wave(path: str) -> np.ndarray:
+    """A ``.wav`` file as the flat float32 waveform ``mfcc()`` is given: int16 scaled by 1/32768, other sample types
+    converted as they are, channels interleaved.  Raises when the file cannot be read."""
+    from scipy.io import wavfile
+    _, wav = wavfile.read(path)
+    return (wav.astype(np.float32) / 32768.0 if wav.dtype == np.int16 else wav.astype(np.float32)).ravel()
 
 
 class SpeechCommandsDataset(Dataset):
@@ -86,10 +107,7 @@ class SpeechCommandsDataset(Dataset):
     def __getitem__(self, i):
         path, name = self.samples[i]
         try:
-            from scipy.io import wavfile
-            sr, wav = wavfile.read(path)
-            wav = wav.astype(np.float32) / 32768.0 if wav.dtype == np.int16 else wav.astype(np.float32)
-            feat = mfcc(wav)
+            feat = mfcc(read_wave(path))
         except Exception:
             feat = np.zeros((N_MFCC, FRAMES), dtype=np.float32)
         return torch.from_numpy(feat), CLASSES.index(name)

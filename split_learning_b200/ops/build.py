@@ -13,7 +13,8 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["umma_gemm.cu", "fused_cut.cu", "elementwise.cu", "transformer.cu", "allreduce.cu", "ticket.cu", "peer.cu"]
+SOURCES = ["umma_gemm.cu", "fused_cut.cu", "elementwise.cu", "transformer.cu", "allreduce.cu", "ticket.cu", "peer.cu",
+           "audio.cu"]
 LIB = os.path.join(HERE, "_slb200.so")
 STAMP = LIB + ".sha"
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

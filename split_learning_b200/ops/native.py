@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import c_float, c_int, c_longlong, c_uint32, c_uint64, c_void_p
+from ctypes import c_double, c_float, c_int, c_longlong, c_uint32, c_uint64, c_void_p
 from typing import Sequence
 
 import torch
@@ -48,7 +48,8 @@ def preload(device=None) -> None:
         return
     with torch.cuda.device(d):
         bad = (lib().slb_preload_gemm() + lib().slb_preload_fused() + lib().slb_preload_elementwise()
-               + lib().slb_preload_transformer() + lib().slb_preload_allreduce() + lib().slb_preload_ticket())
+               + lib().slb_preload_transformer() + lib().slb_preload_allreduce() + lib().slb_preload_ticket()
+               + lib().slb_preload_audio())
     if bad:
         raise NativeError(f"{bad} kernels failed to load (wrong GPU architecture? this library is sm_90a only)")
     _preloaded.add(d)
@@ -687,3 +688,44 @@ def image_batch(data_u8, idx, dx, dy, flip, out, mean, std):
     sd = (c_float * 3)(*([float(v) for v in std] + [1.0] * (3 - len(std))))
     _check(lib().slb_image_batch(_p(data_u8), _p(idx), _p(dx), _p(dy), _p(flip), _p(out), c_int(B), c_int(C), c_int(H), c_int(W),
                                  m, sd, _stream()), "image_batch")
+
+
+# ------------------------------------------------------------------ GPU-resident Speech Commands loader
+def mfcc(waves, valid, out, window, fb, dct, twiddle, hop: int, preemph: float, floor: float):
+    """out fp32 [n, ncoef, frames] = MFCC of the fp32 waveforms [n, L] (L = win + hop * (frames - 1)), computed in fp64 with
+    the fp64 tables window [win], fb [nmels, nfft/2 + 1], dct [ncoef, nmels] and twiddle [nfft, 2] (cos, sin of 2 pi j /
+    nfft).  Clips whose uint8 ``valid`` byte is 0 get zero features.  A refused call launches nothing."""
+    if (waves.dtype != torch.float32 or out.dtype != torch.float32 or valid.dtype != torch.uint8
+            or any(t.dtype != torch.float64 for t in (window, fb, dct, twiddle))):
+        raise NativeError("mfcc: waves / out fp32, valid uint8, tables fp64")
+    if not all(t.is_contiguous() for t in (waves, valid, out, window, fb, dct, twiddle)):
+        raise NativeError("mfcc: tensors must be contiguous")
+    if waves.dim() != 2 or out.dim() != 3 or fb.dim() != 2 or dct.dim() != 2 or twiddle.dim() != 2 or twiddle.shape[1] != 2:
+        raise NativeError("mfcc: waves [n, L], out [n, ncoef, frames], fb [nmels, nbins], dct [ncoef, nmels], twiddle [nfft, 2]")
+    n, L = waves.shape
+    ncoef, frames = out.shape[1], out.shape[2]
+    nfft, nmels = twiddle.shape[0], fb.shape[0]
+    if (out.shape[0] != n or valid.numel() != n or window.numel() > nfft or fb.shape[1] != nfft // 2 + 1
+            or tuple(dct.shape) != (ncoef, nmels)):
+        raise NativeError(f"mfcc: inconsistent shapes waves {tuple(waves.shape)} out {tuple(out.shape)} fb {tuple(fb.shape)} "
+                          f"dct {tuple(dct.shape)} twiddle {tuple(twiddle.shape)}")
+    _check(lib().slb_mfcc(_p(waves), _p(valid), _p(window), _p(fb), _p(dct), _p(twiddle), _p(out), c_int(n), c_int(L),
+                          c_int(window.numel()), c_int(hop), c_int(frames), c_int(nfft), c_int(nmels), c_int(ncoef),
+                          c_double(preemph), c_double(floor), _stream()), "mfcc")
+
+
+def feature_batch(features, labels, idx, out, y):
+    """out [B, ...] fp32 = features[idx], y [B] int64 = labels[idx]: one microbatch of a resident fp32 [N, ...] split
+    (rows of a multiple of 4 floats, 16-byte aligned); idx int64 [B] with every entry in [0, N)."""
+    if features.dtype != torch.float32 or out.dtype != torch.float32 or any(t.dtype != torch.int64 for t in (labels, idx, y)):
+        raise NativeError("feature_batch: features / out fp32, labels / idx / y int64")
+    if not all(t.is_contiguous() for t in (features, labels, idx, out, y)):
+        raise NativeError("feature_batch: tensors must be contiguous")
+    n, b = features.shape[0] if features.dim() else 0, idx.numel()
+    if (labels.numel() != n or out.dim() == 0 or out.shape[0] != b or y.numel() != b
+            or tuple(out.shape[1:]) != tuple(features.shape[1:])):
+        raise NativeError(f"feature_batch: features {tuple(features.shape)} labels {tuple(labels.shape)} idx {tuple(idx.shape)} "
+                          f"out {tuple(out.shape)} y {tuple(y.shape)}")
+    d = features[0].numel() if n else 0
+    _check(lib().slb_feature_batch(_p(features), _p(labels), _p(idx), _p(out), _p(y), c_int(n), c_int(b), c_longlong(d),
+                                   _stream()), "feature_batch")
