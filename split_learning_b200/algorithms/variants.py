@@ -144,7 +144,8 @@ class SequentialServer(Server):
             if self.validation and full:
                 from ..validation import get_val
                 ok, val = get_val(self.model_name, self.data_name, full, self.logger, strict=self.STRICT_VALIDATION,
-                                  native=self.cfg.b200.get("native-validation", False))
+                                  native=self.cfg.b200.get("native-validation", False),
+                                  speech_features=self.cfg.b200.get("speech-features", "engine"))
                 metrics.update(val)
             if ok:
                 if full and self.save_parameters:
@@ -337,7 +338,8 @@ class FlexServer(Server):
                 if self.validation and full:
                     from ..validation import get_val
                     ok, val = get_val(self.model_name, self.data_name, full, self.logger,
-                                      native=self.cfg.b200.get("native-validation", False))
+                                      native=self.cfg.b200.get("native-validation", False),
+                                      speech_features=self.cfg.b200.get("speech-features", "engine"))
                     metrics.update(val)
                 if ok and full:
                     save_checkpoint(full, checkpoint_path(self.model_name, self.data_name, self.workdir))
@@ -484,7 +486,8 @@ class TwoLSServer(Server):
             if self.validation:
                 from ..validation import get_val
                 ok, val = get_val(self.model_name, self.data_name, self.global_model, self.logger,
-                                  native=self.cfg.b200.get("native-validation", False))
+                                  native=self.cfg.b200.get("native-validation", False),
+                                  speech_features=self.cfg.b200.get("speech-features", "engine"))
                 metrics.update(val)
             self.round = self.round - 1 if ok else 0
         else:

@@ -167,7 +167,8 @@ class RpcClient:
             self.train_loader = data_loader(self.data_name, int(self.learning["batch-size"]), self.label_count,
                                             train=True, synthetic=True if self.opts.get("synthetic-data") else None,
                                             seed=zlib.crc32(str(self.client_id).encode()) & 0x7FFFFFFF,   # every client its own samples
-                                            device=self.device, gpu_loader=bool(self.opts.get("gpu-loader", False)))
+                                            device=self.device, gpu_loader=bool(self.opts.get("gpu-loader", False)),
+                                            speech_features=self.opts.get("speech-features", "engine"))
         self.is_first, self.is_last = is_first, is_last
         self.start_msg = msg
         self.send_to_server(M.ready(self.client_id, self.layer_id))

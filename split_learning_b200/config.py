@@ -38,6 +38,7 @@ DEFAULT_B200 = {
     "routing": "round-robin",      # competing-consumer emulation on the device plane
     "data-plane": "host",          # host = broker queues (any device) | device = peer-memory mailboxes (CUDA)
     "native-validation": False,    # false = torch modules | true = native eval plan (error if unsupported) | auto
+    "speech-features": "engine",   # Speech Commands MFCC recipe: engine | reference (the reference's compute_mfcc)
 }
 
 
@@ -235,6 +236,8 @@ def normalize(raw: Dict[str, Any]) -> Config:
 
 
 def _validate(cfg: Config) -> None:
+    from .data.speechcommands import speech_recipe
+    cfg.b200["speech-features"] = speech_recipe(cfg.b200.get("speech-features"))
     if len(cfg.clients) < 1 or any(c < 0 for c in cfg.clients):
         raise ValueError(f"server.clients must be a list of non-negative ints, got {cfg.clients}")
     n_cut = len(cfg.clients) - 1

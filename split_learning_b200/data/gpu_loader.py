@@ -8,8 +8,9 @@ written as the fp32 NCHW stage input.  No host work and no H2D copy per step; th
 every executor and the device data plane accept as they are.
 
 Speech Commands (KWT) is held as its MFCC features: the host reads each ``.wav`` once, ``mfcc_kernel`` turns the clips into
-[40, 98] features in fp64 with the tables of ``speechcommands.mfcc()`` (the same values the host loader computes per
-``__getitem__``), and each microbatch is one gather (``GpuFeatureLoader``, ``feature_batch_kernel``).
+[40, 98] features in fp64 with the tables of ``speechcommands.mfcc()`` or, with ``b200.speech-features: reference``,
+``mfcc_reference()`` (the same values the host loader computes per ``__getitem__``), and each microbatch is one gather
+(``GpuFeatureLoader``, ``feature_batch_kernel``).
 """
 from __future__ import annotations
 
@@ -103,19 +104,23 @@ class GpuFeatureLoader:
             yield self.batch(order[k * self.batch_size:(k + 1) * self.batch_size])
 
 
-def mfcc_tables(device):
-    """``speechcommands.mfcc_tables()`` as fp64 device tensors (the kernel's window, filterbank, DCT and twiddles)."""
+def mfcc_tables(device, recipe: str = "engine"):
+    """``speechcommands.mfcc_tables(recipe)`` as fp64 device tensors (the kernel's window, filterbank, DCT and twiddles)."""
     from .speechcommands import mfcc_tables as host_tables
-    return {k: torch.from_numpy(v).to(device=device, dtype=torch.float64).contiguous() for k, v in host_tables().items()}
+    return {k: torch.from_numpy(v).to(device=device, dtype=torch.float64).contiguous() for k, v in host_tables(recipe).items()}
 
 
-def mfcc_features(waves: torch.Tensor, valid: torch.Tensor, tables: dict, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """fp32 [n, 40, 98] MFCC features of fp32 waveforms [n, L] (already padded or truncated to L) on the GPU, one
-    ``mfcc`` launch; clips with ``valid == 0`` get zeros, as ``SpeechCommandsDataset`` gives unreadable files."""
-    from .speechcommands import FRAMES, HOP, LOG_FLOOR, N_MFCC, PREEMPH
+def mfcc_features(waves: torch.Tensor, valid: torch.Tensor, tables: dict, out: Optional[torch.Tensor] = None,
+                  recipe: str = "engine") -> torch.Tensor:
+    """fp32 [n, 40, 98] MFCC features of fp32 waveforms [n, L] (already padded or truncated to the recipe's
+    ``clip_length``) on the GPU, one ``mfcc`` launch with the recipe's ``tables``; clips with ``valid == 0`` get zeros, as
+    ``SpeechCommandsDataset`` gives unreadable files."""
+    from .speechcommands import FRAMES, HOP, LOG_FLOOR, N_MFCC, PREEMPH, REF_LOG_EPS, speech_recipe
+    recipe = speech_recipe(recipe)
     if out is None:
         out = torch.empty(waves.shape[0], N_MFCC, FRAMES, dtype=torch.float32, device=waves.device)
-    N.mfcc(waves, valid, out, tables["window"], tables["fb"], tables["dct"], tables["twiddle"], HOP, PREEMPH, LOG_FLOOR)
+    N.mfcc(waves, valid, out, tables["window"], tables["fb"], tables["dct"], tables["twiddle"], HOP, PREEMPH,
+           LOG_FLOOR if recipe == "engine" else REF_LOG_EPS, recipe)
     return out
 
 

@@ -5,7 +5,8 @@ Real datasets follow the reference's recipes (src/dataset/dataloader.py):
     ``distribution[label]`` indices; shuffle; test batch 100  (:61-92)
   * MNIST    — ToTensor + Normalize (variants)
   * AGNEWS   — CSV + BertTokenizer('bert-base-cased'), max_len 128  (:16-59)
-  * SPEECHCOMMANDS — 10-class subset, NumPy MFCC 40x98  (:95-122)
+  * SPEECHCOMMANDS — 10-class subset, NumPy MFCC 40x98  (:95-122); ``speech_features`` ("engine" | "reference",
+    ``b200.speech-features``) picks the MFCC recipe of the training and test loaders (data/speechcommands.py)
 They need files under ``./data`` (no network here).  When the files are missing, or
 ``synthetic=True`` / ``SLB200_SYNTHETIC=1``, a ``SyntheticDataset`` with the same tensor
 shapes, dtypes and per-label counts is used instead (what ``bench.py`` uses).
@@ -167,9 +168,9 @@ def _agnews(batch_size, distribution, train, root="./data"):
     return DataLoader(ds, batch_size=batch_size if train else 20, shuffle=train)
 
 
-def _speechcommands(batch_size, distribution, train, root="./data"):
+def _speechcommands(batch_size, distribution, train, root="./data", recipe="engine"):
     from .speechcommands import CLASSES, SpeechCommandsDataset
-    ds = SpeechCommandsDataset(root=root, subset="training" if train else "testing")
+    ds = SpeechCommandsDataset(root=root, subset="training" if train else "testing", recipe=recipe)
     if not train:
         return DataLoader(ds, batch_size=20, shuffle=False)
     if distribution is None:
@@ -222,19 +223,21 @@ def gpu_image_loader(name: str, batch_size: int, distribution: Sequence[int], de
 SPEECH_CHUNK = 2048      # clips per upload + ``mfcc`` launch while a resident Speech Commands split is built (~130 MB)
 
 
-def speech_features(paths: Sequence[str], device, chunk: int = SPEECH_CHUNK, timing: Optional[dict] = None) -> torch.Tensor:
-    """fp32 [len(paths), 40, 98] device tensor of the MFCC features ``SpeechCommandsDataset.__getitem__`` gives these files:
-    the host reads and converts each file as it does (``read_wave``), pads or truncates it to L = 15 920 samples, and
-    every ``chunk`` clips go to the GPU for one ``mfcc`` launch.  Only the features stay resident; unreadable files get zero
-    rows.  ``timing``: accumulates ``host_s`` (file reads) and ``mfcc_ms`` (kernel time, CUDA events)."""
+def speech_features(paths: Sequence[str], device, chunk: int = SPEECH_CHUNK, timing: Optional[dict] = None,
+                    recipe: str = "engine") -> torch.Tensor:
+    """fp32 [len(paths), 40, 98] device tensor of the MFCC features ``SpeechCommandsDataset(recipe=recipe).__getitem__``
+    gives these files: the host reads and converts each file as it does (``read_wave``), pads or truncates it to the
+    recipe's clip length (15 920 or 16 000 samples), and every ``chunk`` clips go to the GPU for one ``mfcc`` launch.  Only
+    the features stay resident; unreadable files get zero rows.  ``timing``: accumulates ``host_s`` (file reads) and
+    ``mfcc_ms`` (kernel time, CUDA events)."""
     import time
 
     import numpy as np
     from .gpu_loader import mfcc_features, mfcc_tables
-    from .speechcommands import FRAMES, HOP, N_MFCC, WIN, read_wave
+    from .speechcommands import FRAMES, N_MFCC, clip_length, read_wave
     dev = torch.device(device)
-    L = WIN + HOP * (FRAMES - 1)
-    tables = mfcc_tables(dev)
+    L = clip_length(recipe)
+    tables = mfcc_tables(dev, recipe)
     feats = torch.empty(len(paths), N_MFCC, FRAMES, dtype=torch.float32, device=dev)
     for lo in range(0, len(paths), chunk):
         part = paths[lo:lo + chunk]
@@ -243,7 +246,7 @@ def speech_features(paths: Sequence[str], device, chunk: int = SPEECH_CHUNK, tim
         valid = np.ones(len(part), dtype=np.uint8)
         for r, path in enumerate(part):
             try:
-                w = read_wave(path)[:L]
+                w = read_wave(path, recipe)[:L]
             except Exception:
                 valid[r] = 0
                 continue
@@ -254,7 +257,7 @@ def speech_features(paths: Sequence[str], device, chunk: int = SPEECH_CHUNK, tim
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if timing is not None else None
         if ev:
             ev[0].record()
-        mfcc_features(wd, vd, tables, out=feats[lo:lo + len(part)])
+        mfcc_features(wd, vd, tables, out=feats[lo:lo + len(part)], recipe=recipe)
         if ev:
             ev[1].record()
             ev[1].synchronize()
@@ -263,10 +266,10 @@ def speech_features(paths: Sequence[str], device, chunk: int = SPEECH_CHUNK, tim
 
 
 def speech_gpu_loader(batch_size: int, distribution: Sequence[int], device, synthetic: bool, root: str = "./data",
-                      seed: int = 0):
+                      seed: int = 0, recipe: str = "engine"):
     """Speech Commands training loader whose split lives on the GPU as MFCC features (``GpuFeatureLoader``): real data takes
-    the sample list and per-label subset of ``_speechcommands`` and computes the features once (``speech_features``);
-    synthetic data uploads the samples of the host synthetic loader."""
+    the sample list and per-label subset of ``_speechcommands`` and computes the features once in the MFCC ``recipe``
+    (``speech_features``); synthetic data uploads the samples of the host synthetic loader."""
     from .gpu_loader import GpuFeatureLoader
     if synthetic:
         ds = SyntheticDataset("SPEECHCOMMANDS", distribution, seed=seed)
@@ -275,7 +278,7 @@ def speech_gpu_loader(batch_size: int, distribution: Sequence[int], device, synt
     ds = SpeechCommandsDataset(root=root, subset="training")
     labels = [CLASSES.index(name) for _, name in ds.samples]
     pick = _select_by_label(labels, distribution)
-    feats = speech_features([ds.samples[i][0] for i in pick], device)
+    feats = speech_features([ds.samples[i][0] for i in pick], device, recipe=recipe)
     return GpuFeatureLoader(feats, torch.tensor([labels[i] for i in pick], dtype=torch.long), batch_size, device, seed=seed)
 
 
@@ -317,10 +320,14 @@ def resident_test_loader(data_name: str, device, synthetic: Optional[bool] = Non
 def data_loader(data_name: Optional[str] = None, batch_size: Optional[int] = None,
                 distribution: Optional[Sequence[int]] = None, train: bool = True,
                 synthetic: Optional[bool] = None, root: str = "./data", seed: int = 0, device=None,
-                gpu_loader: bool = False) -> DataLoader:
+                gpu_loader: bool = False, speech_features: str = "engine") -> DataLoader:
+    """``speech_features``: the MFCC recipe of real Speech Commands data, "engine" or "reference"
+    (``b200.speech-features``); synthetic data and the other datasets ignore it."""
+    from .speechcommands import speech_recipe
     name = str(data_name).upper()
     if name not in DATASET_SHAPES:
         raise ValueError(f"Dataset {data_name} not supported.")
+    recipe = speech_recipe(speech_features)
     explicit = synthetic is not None or os.environ.get("SLB200_SYNTHETIC", "0") == "1"
     if synthetic is None:
         synthetic = _synthetic_default(name, root)
@@ -340,11 +347,13 @@ def data_loader(data_name: Optional[str] = None, batch_size: Optional[int] = Non
         return gpu_image_loader(name, int(batch_size), distribution, device, bool(synthetic), root, seed)
     if (gpu_loader and train and name == "SPEECHCOMMANDS" and device is not None and torch.device(device).type == "cuda"
             and distribution is not None and len(distribution) > 0):
-        return speech_gpu_loader(int(batch_size), distribution, device, bool(synthetic), root, seed)
+        return speech_gpu_loader(int(batch_size), distribution, device, bool(synthetic), root, seed, recipe)
     if synthetic or name not in _REAL:
         shape, dtype, ncls, test_bs = DATASET_SHAPES[name]
         if distribution is None or len(distribution) == 0:
             distribution = [max(1, (100 if not train else 500) // ncls)] * ncls
         pin = train and device is not None and torch.device(device).type == "cuda"
         return synthetic_loader(name, batch_size if train else test_bs, distribution, train=train, seed=seed, pin=pin)
+    if name == "SPEECHCOMMANDS":
+        return _speechcommands(batch_size, distribution, train, root, recipe)
     return _REAL[name](batch_size, distribution, train, root)

@@ -12,6 +12,12 @@
 //                          from the same arrays mfcc() uses, and the frame geometry is a launch argument: the kernel holds
 //                          no recipe constant of its own.  One CTA per (clip, group of MFCC_GROUP frames); one thread per
 //                          frequency bin.  Clips whose valid byte is 0 (files the host could not read) get zero features.
+//                          The template argument is the recipe (b200.speech-features).  MFCC_REFERENCE follows
+//                          speechcommands.mfcc_reference() instead, in its two steps that differ:
+//                            pre-emphasis        in fp32, p[t] = w[t] - (float)a * w[t-1] (each operation rounded), as NumPy
+//                                                computes it on a float32 waveform; widened to fp64 for the window
+//                            mel + log           20 log10(e), e = fb @ power, with e == 0 replaced by floor (eps)
+//                          MFCC_ENGINE compiles to the code the kernel had before it took a recipe.
 //   feature_batch_kernel   one training microbatch gathered from the resident features: out[b] = feat[idx[b]],
 //                          y[b] = labels[idx[b]], 16-byte loads and stores.
 #include "sm90.cuh"
@@ -21,6 +27,7 @@ namespace slb {
 constexpr int MFCC_GROUP = 7;            // frames per CTA: 98 = 14 x 7; every twiddle load feeds 2 x 7 FMAs
 constexpr int MFCC_XS = 8;               // row pitch (doubles) of the staged frame samples: 4 x 16-byte loads per sample
 constexpr int MFCC_MAX_THREADS = 512;
+enum MfccRecipe : int { MFCC_ENGINE = 0, MFCC_REFERENCE = 1 };   // the recipe argument of slb_mfcc
 
 struct MfccArgs {
   const float* waves;
@@ -32,7 +39,7 @@ struct MfccArgs {
   float* out;                            // [n][ncoef][frames]
   int n, L, win, hop, frames, nfft, nbins, nmels, ncoef;
   int span;                              // floats of raw waveform staged per CTA (multiple of 4)
-  double preemph, floor;
+  double preemph, floor;                 // floor: lower clamp of the mel energies (engine), value of exact zeros (reference)
 };
 
 // dynamic shared memory of one CTA: twiddles, frame samples, raw fp32 span, power spectra, mel energies
@@ -41,6 +48,7 @@ static inline size_t mfcc_smem(int nfft, int win, int nbins, int nmels, int span
          + sizeof(float) * span;
 }
 
+template <MfccRecipe R>
 __global__ void __launch_bounds__(MFCC_MAX_THREADS) mfcc_kernel(const MfccArgs a) {
   pdl_trigger();
   pdl_wait();
@@ -80,8 +88,14 @@ __global__ void __launch_bounds__(MFCC_MAX_THREADS) mfcc_kernel(const MfccArgs a
     double v = 0.0;
     if (f < gf) {
       const int s = (f0 + f) * a.hop + t;
-      const double x = static_cast<double>(raw[s - s0]);
-      const double p = s == 0 ? x : __dsub_rn(x, __dmul_rn(a.preemph, static_cast<double>(raw[s - 1 - s0])));
+      double p;
+      if constexpr (R == MFCC_ENGINE) {
+        const double x = static_cast<double>(raw[s - s0]);
+        p = s == 0 ? x : __dsub_rn(x, __dmul_rn(a.preemph, static_cast<double>(raw[s - 1 - s0])));
+      } else {
+        const float x = raw[s - s0];
+        p = static_cast<double>(s == 0 ? x : __fsub_rn(x, __fmul_rn(static_cast<float>(a.preemph), raw[s - 1 - s0])));
+      }
       v = __dmul_rn(p, a.window[t]);
     }
     xw[i] = v;
@@ -129,7 +143,12 @@ __global__ void __launch_bounds__(MFCC_MAX_THREADS) mfcc_kernel(const MfccArgs a
     for (int k = lane; k < a.nbins; k += 32) s = fma(pr[k], __ldg(fr + k), s);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) mel[f * a.nmels + m] = log(fmax(s, a.floor));
+    if (lane == 0) {
+      if constexpr (R == MFCC_ENGINE)
+        mel[f * a.nmels + m] = log(fmax(s, a.floor));
+      else
+        mel[f * a.nmels + m] = 20.0 * log10(s == 0.0 ? a.floor : s);
+    }
   }
   __syncthreads();
 
@@ -173,11 +192,14 @@ using namespace slb;
 
 extern "C" {
 
-// Returns -3 (shape) or -4 (alignment) without launching anything.  L = win + hop * (frames - 1) and L % 4 == 0
-// (16-byte waveform loads); win <= nfft, nfft even, nfft / 2 + 1 bins; waves 16-byte aligned, tables 8 (twiddle 16).
+// Returns -3 (shape, recipe) or -4 (alignment) without launching anything.  L = win + hop * (frames - 1) and L % 4 == 0
+// (16-byte waveform loads); win <= nfft, nfft even, nfft / 2 + 1 bins; waves 16-byte aligned, tables 8 (twiddle 16);
+// recipe MFCC_ENGINE or MFCC_REFERENCE.  Dynamic shared memory (mfcc_smem): 55,880 B for the engine geometry (400 / 512),
+// 59,912 B for the reference geometry (480 / 480).
 int slb_mfcc(const float* waves, const uint8_t* valid, const double* window, const double* fb, const double* dct,
              const void* twiddle, float* out, int n, int L, int win, int hop, int frames, int nfft, int nmels, int ncoef,
-             double preemph, double floor, cudaStream_t st) {
+             double preemph, double floor, int recipe, cudaStream_t st) {
+  if (recipe != MFCC_ENGINE && recipe != MFCC_REFERENCE) return -3;
   if (n < 1 || win < 1 || hop < 1 || frames < 1 || nmels < 1 || ncoef < 1 || nfft < 2 || (nfft & 1) || win > nfft) return -3;
   if (static_cast<long long>(win) + static_cast<long long>(hop) * (frames - 1) != L || (L & 3)) return -3;
   const int groups = (frames + MFCC_GROUP - 1) / MFCC_GROUP;
@@ -193,11 +215,12 @@ int slb_mfcc(const float* waves, const uint8_t* valid, const double* window, con
   a.span = ((MFCC_GROUP - 1) * hop + win + 1 + 3 + 3) & ~3;     // predecessor sample + alignment of both ends
   const size_t smem = mfcc_smem(nfft, win, a.nbins, nmels, a.span);
   if (smem > 227 * 1024) return -3;
+  void (*kernel)(MfccArgs) = recipe == MFCC_ENGINE ? mfcc_kernel<MFCC_ENGINE> : mfcc_kernel<MFCC_REFERENCE>;
   if (smem > 48 * 1024 &&
-      cudaFuncSetAttribute(mfcc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess)
+      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess)
     return launch_status();
   const int threads = min(MFCC_MAX_THREADS, (a.nbins + 31) & ~31);
-  launch_k(mfcc_kernel, dim3(static_cast<unsigned>(n * groups)), dim3(threads), smem, st, a);
+  launch_k(kernel, dim3(static_cast<unsigned>(n * groups)), dim3(threads), smem, st, a);
   return launch_status();
 }
 
@@ -216,7 +239,8 @@ int slb_feature_batch(const float* feat, const long long* labels, const long lon
 int slb_preload_audio() {
   cudaFuncAttributes a;
   int bad = 0;
-  bad += cudaFuncGetAttributes(&a, mfcc_kernel) != cudaSuccess;
+  bad += cudaFuncGetAttributes(&a, mfcc_kernel<MFCC_ENGINE>) != cudaSuccess;
+  bad += cudaFuncGetAttributes(&a, mfcc_kernel<MFCC_REFERENCE>) != cudaSuccess;
   bad += cudaFuncGetAttributes(&a, feature_batch_kernel) != cudaSuccess;
   return bad;
 }

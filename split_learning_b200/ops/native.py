@@ -691,10 +691,17 @@ def image_batch(data_u8, idx, dx, dy, flip, out, mean, std):
 
 
 # ------------------------------------------------------------------ GPU-resident Speech Commands loader
-def mfcc(waves, valid, out, window, fb, dct, twiddle, hop: int, preemph: float, floor: float):
+MFCC_RECIPES = {"engine": 0, "reference": 1}          # MfccRecipe of audio.cu
+
+
+def mfcc(waves, valid, out, window, fb, dct, twiddle, hop: int, preemph: float, floor: float, recipe: str = "engine"):
     """out fp32 [n, ncoef, frames] = MFCC of the fp32 waveforms [n, L] (L = win + hop * (frames - 1)), computed in fp64 with
     the fp64 tables window [win], fb [nmels, nfft/2 + 1], dct [ncoef, nmels] and twiddle [nfft, 2] (cos, sin of 2 pi j /
-    nfft).  Clips whose uint8 ``valid`` byte is 0 get zero features.  A refused call launches nothing."""
+    nfft).  Clips whose uint8 ``valid`` byte is 0 get zero features.  ``recipe``: "engine" (fp64 pre-emphasis,
+    ln(max(e, floor))) or "reference" (fp32 pre-emphasis, 20 log10(e) with e == 0 replaced by floor).  A refused call
+    launches nothing."""
+    if recipe not in MFCC_RECIPES:
+        raise NativeError(f"mfcc: recipe must be one of {sorted(MFCC_RECIPES)}, got {recipe!r}")
     if (waves.dtype != torch.float32 or out.dtype != torch.float32 or valid.dtype != torch.uint8
             or any(t.dtype != torch.float64 for t in (window, fb, dct, twiddle))):
         raise NativeError("mfcc: waves / out fp32, valid uint8, tables fp64")
@@ -711,7 +718,7 @@ def mfcc(waves, valid, out, window, fb, dct, twiddle, hop: int, preemph: float, 
                           f"dct {tuple(dct.shape)} twiddle {tuple(twiddle.shape)}")
     _check(lib().slb_mfcc(_p(waves), _p(valid), _p(window), _p(fb), _p(dct), _p(twiddle), _p(out), c_int(n), c_int(L),
                           c_int(window.numel()), c_int(hop), c_int(frames), c_int(nfft), c_int(nmels), c_int(ncoef),
-                          c_double(preemph), c_double(floor), _stream()), "mfcc")
+                          c_double(preemph), c_double(floor), c_int(MFCC_RECIPES[recipe]), _stream()), "mfcc")
 
 
 def feature_batch(features, labels, idx, out, y):

@@ -472,7 +472,8 @@ class Server:
             if self.validation and full:
                 from .validation import get_val
                 ok, val = get_val(self.model_name, self.data_name, full, self.logger,
-                                  native=self.cfg.b200.get("native-validation", False))
+                                  native=self.cfg.b200.get("native-validation", False),
+                                  speech_features=self.cfg.b200.get("speech-features", "engine"))
                 metrics.update(val)
             if ok:
                 if full:

@@ -102,7 +102,9 @@ def _native_evaluate(klass, model_name, data_name, state_dict_full, device, pump
 
 def get_val(model_name: str, data_name: str, state_dict_full, logger=None, strict: bool = False,
             device: Optional[str] = None, pump=None, synthetic: Optional[bool] = None,
-            native=False) -> Tuple[bool, Dict[str, float]]:
+            native=False, speech_features: str = "engine") -> Tuple[bool, Dict[str, float]]:
+    """``speech_features``: the Speech Commands MFCC recipe of the test loader (``b200.speech-features``); it must be the
+    recipe the model was trained on."""
     try:
         klass = get_model_class(model_name, data_name)
     except ValueError:
@@ -129,7 +131,7 @@ def get_val(model_name: str, data_name: str, state_dict_full, logger=None, stric
         model = klass()
         model.load_state_dict(state_dict_full)
         model.to(device)
-        loader = data_loader(data_name=data_name, train=False, synthetic=synthetic)
+        loader = data_loader(data_name=data_name, train=False, synthetic=synthetic, speech_features=speech_features)
         m = evaluate(model, loader, device, pump)
     m["val_backend"] = backend
     line = "Test set:Loss: {:.4f}; Accuracy: {}/{} ({:.2f}%)\n".format(

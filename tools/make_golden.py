@@ -3,7 +3,8 @@
 The tests compare this engine with the reference implementation it reproduces; they read these files instead of the
 reference tree, so the suite runs from a plain checkout.
 
-    python tools/make_golden.py cpu REFERENCE_DIR        # configs, planning / FedAvg oracles, model layouts and outputs
+    python tools/make_golden.py cpu REFERENCE_DIR        # configs, planning / FedAvg oracles, model layouts and outputs,
+                                                         # Speech Commands MFCC features (speech_mfcc_reference.npz)
     SLB200_REFERENCE_DIR=REFERENCE_DIR python baseline/install_reference.py   # reference trainers -> baseline/_ref
     python tools/make_golden.py parity [OUT_DIR]         # reference trainers on a GPU: TF32 run + fp32 oracle (CUDA)
 """
@@ -86,7 +87,50 @@ def cpu(ref):
                 forwards[cls] = t(x).tolist()
     with open(os.path.join(GOLDEN, "models.json"), "w") as f:
         json.dump({"layouts": layouts, "forward": forwards}, f, indent=0)
+    speech(ref)
     print("wrote", GOLDEN)
+
+
+def speech_clips() -> dict:
+    """Deterministic test clips in the sample types a ``.wav`` file holds: full length, padded (9 000) and truncated
+    (17 000)."""
+    rng = np.random.default_rng(2024)
+    t = np.arange(16000) / 16000.0
+    return {
+        "chirp": (0.6 * np.sin(2 * np.pi * (60.0 + 3900.0 * t) * t)).astype(np.float32),
+        "noise": (rng.standard_normal(16000) * 0.1).astype(np.float32),
+        "square": np.where((np.arange(16000) // 40) % 2 == 0, 32767, -32768).astype(np.int16),
+        "silence": np.zeros(16000, np.float32),
+        "tone_int32": (np.sin(2 * np.pi * 440.0 * t) * 2.0 ** 30).astype(np.int32),
+        "pad_int32": (rng.standard_normal(9000) * 2.0 ** 27).astype(np.int32),
+        "trunc_int16": (rng.standard_normal(17000) * 3000).clip(-32768, 32767).astype(np.int16),
+    }
+
+
+def speech(ref):
+    """``tests/golden/speech_mfcc_reference.npz``: the reference recipe's MFCC features, from the reference itself.
+      clip/NAME      the input clips (int16 / int32 / float32)
+      mfcc/NAME      fp64 ``compute_mfcc`` of each clip, converted and padded or truncated to 16 000 samples as the
+                     reference's ``SpeechCommandsDataset.__getitem__`` does
+      item/RELPATH   fp32 ``__getitem__`` features of every mono file of ``tests/speech_tree.py``'s tree (per_class 1)"""
+    import tempfile
+    from speech_tree import make_tree
+    mod = _import_from(ref, "src.dataset.SPEECHCOMMANDS")
+    data = {}
+    for name, c in speech_clips().items():
+        w = c.astype(np.float32) / {np.dtype(np.int16): 32768.0, np.dtype(np.int32): 2147483648.0}.get(c.dtype, 1.0)
+        w = np.pad(w, (0, max(0, 16000 - w.size)))[:16000]
+        data[f"clip/{name}"] = c
+        data[f"mfcc/{name}"] = np.asarray(mod.compute_mfcc(w, sample_rate=16000, n_mfcc=40), dtype=np.float64)
+    with tempfile.TemporaryDirectory() as root:
+        tree = make_tree(root, per_class=1)
+        with contextlib.redirect_stdout(io.StringIO()):
+            ds = mod.SpeechCommandsDataset(root=root, subset="training")
+            for i, (path, _) in enumerate(ds.samples):
+                rel = os.path.relpath(path, tree["base"]).replace(os.sep, "/")
+                if rel != tree["stereo"]:                 # the reference gives a multi-channel file a wrongly shaped tensor
+                    data[f"item/{rel}"] = ds[i][0].numpy()
+    np.savez_compressed(os.path.join(GOLDEN, "speech_mfcc_reference.npz"), **dict(sorted(data.items())))
 
 
 def _reference_run(batches, device, cut, learning, tf32):
